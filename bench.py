@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — rays/s of the HOLD foreground hot path (SURVEY.md §8d metric) on N B200s.
+"""bench.py — rays/s of the HOLD foreground hot path (SURVEY.md §8d metric) on N H100s.
 
 One "step" = one 512x512 frame (262 144 rays) of BASELINE.json configs[1] (right hand + rigid object,
 "128 samples/ray" = N_samples_eval 128 / N_samples 64 / N_samples_extra 32, density beta 0.03 so that the
@@ -9,6 +9,7 @@ feature, skinning Jacobian, colour net, density) -> n-way merge + volume integra
 
   python bench.py --gpus N --steps K --warmup W            # ours (torchrun for N > 1)
   python bench.py --impl reference [--steps K]             # the reference algorithm on the host CPU cores
+  python bench.py --steps K --dump-outputs DIR             # also write the last timed step's outputs as DIR/<name>.npy
 
 Rays shard over ranks with no data-path collective (render.py has no gradients, SURVEY D4): each rank renders
 its own frames -> "scaling": "weak".  Timing: CUDA events around exactly K steps, barrier + synchronize on
@@ -49,16 +50,20 @@ def flops_per_ray(rounds: int, nodes=NODES, n_eval=S, s_final=S // 2 + S // 4 + 
     return tot
 
 
+# NVIDIA's data sheet for the H100 SXM (700 W): 989 TFLOP/s dense FP16 / BF16.  A card run at a lower power limit sustains less.
+H100_FP16_DENSE_TFLOPS = 989.0
+
+
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 1590.0, 1400.0, "fallback"
+        return d.get("bf16_tflops", H100_FP16_DENSE_TFLOPS), d.get("bf16_tflops_sustained", H100_FP16_DENSE_TFLOPS), "MEASURED_PEAKS.json bf16_tflops"
+    return H100_FP16_DENSE_TFLOPS, H100_FP16_DENSE_TFLOPS, "H100 SXM data sheet, dense FP16 at 700 W"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index=0):
         super().__init__(daemon=True)
@@ -132,8 +137,8 @@ def usable_cpus() -> int:
 def cpu_reference_rays_per_s(n_rays_per_worker: int = 1024, repeats: int = 1, threads: int | None = None, workers: int | None = None):
     """The reference's algorithm (oracle port, pinned to the reference modules by oracle/ref_harness.py) on ALL host cores:
     rays are independent, so the frame's 512-ray chunks (datasets/eval_datasets.py:13) are farmed over `workers` processes of
-    `threads` torch threads each (one process tops out at ~16 threads on these small GEMMs: sweep on the round-1 box, 2 x Xeon
-    8562Y+: 16 threads 105 rays/s, 32: 89, 64: 56, 128: 0.84).  Wall clock from a common start barrier to the last worker's end."""
+    `threads` torch threads each (one process gains nothing beyond ~16 threads on these small GEMMs; HOLD_CPU_THREADS /
+    HOLD_CPU_WORKERS override the split).  Wall clock from a common start barrier to the last worker's end."""
     import multiprocessing as mp
 
     ncpu = usable_cpus()
@@ -159,7 +164,7 @@ def _cpu_line(rps, cores, dt, info, steps):
     return {"value": rps, "unit": "rays/s", "cores": cores, "kind": "port",
             "sample": f"{info['rays']} rays of the same 512x512 workload ({info['workers']} processes x {info['threads_per_worker']} threads, "
                       f"disjoint 512-ray chunks, {steps} pass(es); {info.get('usable_cpus')} usable hardware threads of {info.get('os_cpu_count')}) in {dt:.1f} s wall; oracle/hold_oracle.py = torch-CPU fp32 restatement pinned "
-                      f"to the reference's own modules (oracle/ref_harness.py; /root/reference cannot travel to the GPU box, hence 'port')"}
+                      f"to the reference's own modules (oracle/ref_harness.py; the reference itself is not part of this repository, hence 'port')"}
 
 
 def run_reference(args):
@@ -167,7 +172,7 @@ def run_reference(args):
     if rank != 0:
         return
     reps = max(1, args.steps)
-    # one 512-ray chunk per worker and step: ~5 s per step on the GPU box's host, so that --steps 20 ends within a few minutes
+    # one 512-ray chunk per worker and step, so that --steps 20 ends within a few minutes on a host with a few dozen cores
     rps, cores, dt, info = cpu_reference_rays_per_s(512, repeats=reps)
     line = {
         "impl": "reference", "metric": "rays/sec (128 samples/ray)", "value": rps, "unit": "rays/s", "n_gpus": args.gpus,
@@ -182,30 +187,32 @@ def run_reference(args):
     print(json.dumps(line))
 
 
-def ncu_traffic_bytes():
-    """dram__bytes_read.sum + dram__bytes_write.sum of the dominant launch from the newest committed ncu --set full capture
-    (profiles/r*_ncu_k_mlp_tc0*_raw.csv), or None."""
-    import csv
-    import glob
+DUMP_LIMIT_BYTES = 64 << 20
 
-    cands = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_ncu_k_mlp_tc0*raw.csv")))
-    for path in reversed(cands):
-        try:
-            rows = list(csv.reader(open(path)))
-            hdr, units = rows[0], rows[1]
-            for r in rows[2:]:
-                d = dict(zip(hdr, r))
-                if "k_mlp_tc" not in d.get("Kernel Name", ""):
-                    continue
-                tot = 0.0
-                for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                    u = units[hdr.index(k)].lower()
-                    mult = {"byte": 1.0, "kbyte": 1e3, "mbyte": 1e6, "gbyte": 1e9}[u]
-                    tot += float(d[k]) * mult
-                return tot, os.path.basename(path)
-        except Exception:
+
+def dump_outputs(out, d, n_rays):
+    """The arrays forward_fg returned for the last timed frame, one DIR/<name>.npy each (floating point as float32 / float64,
+    integer counters as float64).  Above DUMP_LIMIT_BYTES in all, the per-ray arrays keep a fixed, seeded sample of rays
+    (their indices in ray_sample.npy)."""
+    import numpy as np
+
+    arrs = {}
+    for k, v in out.items():
+        if not torch.is_tensor(v) or v.numel() == 0:
             continue
-    return None, None
+        v = v.detach()
+        v = v.double() if (v.dtype == torch.float64 or not v.is_floating_point()) else v.float()
+        arrs[k] = v.cpu().numpy()
+    if sum(a.nbytes for a in arrs.values()) > DUMP_LIMIT_BYTES:
+        per_ray = sum(a.nbytes for a in arrs.values() if a.ndim and a.shape[0] == n_rays) / n_rays
+        rest = sum(a.nbytes for a in arrs.values() if not (a.ndim and a.shape[0] == n_rays))
+        keep = int((DUMP_LIMIT_BYTES - rest - 8 * n_rays) // max(per_ray, 1.0))
+        idx = np.sort(torch.randperm(n_rays, generator=torch.Generator().manual_seed(0))[:keep].numpy())
+        arrs = {k: (a[idx] if a.ndim and a.shape[0] == n_rays else a) for k, a in arrs.items()}
+        arrs["ray_sample"] = idx.astype(np.float64)
+    os.makedirs(d, exist_ok=True)
+    for k, a in arrs.items():
+        np.save(os.path.join(d, f"{k}.npy"), a)
 
 
 def run_train(args):
@@ -309,7 +316,7 @@ def run_train(args):
             "config": {"workload": f"configs[4] / SURVEY C5: training step, {Bf} frames x {px} pixels per rank, right hand + object, 128 samples/ray, beta {BETA}",
                        "collective": f"one flat-bucket all-reduce of {n_grad} fp32 gradients per step (NCCL)" if world > 1 else "none (1 rank)",
                        "losses": "L1 rgb + L2 semantics + eikonal (256 canonical samples per frame)", "model": "right hand + object + NeRF++ background (32 inverse-sphere samples/ray)",
-                       "mlp_mode": "tcgen05 fp16-split x3: hold_linear (activations), hold_wgrad (weight gradients); hold_composite_bwd"},
+                       "mlp_mode": "wgmma fp16-split x3: hold_linear (activations), hold_wgrad (weight gradients); hold_composite_bwd"},
             "gpu_launches": launches_per_step * args.steps, "launch_mode": graph_note, "loss": float(loss), "loss_terms": {k: float(v) for k, v in parts.items()}}))
     if dist is not None:
         dist.destroy_process_group()
@@ -325,8 +332,10 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--graph", action="store_true", help="--config train: capture the step as one CUDA graph and time replays")
     ap.add_argument("--config", default="render", choices=["render", "train"],
-                    help="render: BASELINE configs[1] (the driver's line); train: one data-parallel training step (configs[4] / SURVEY C5)")
+                    help="render: BASELINE configs[1] (the default line); train: one data-parallel training step (configs[4] / SURVEY C5)")
     ap.add_argument("--no-extras", action="store_true", help="skip the configs[2] (two hands + object) and full-forward (with background) fields")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="render: write the outputs of the last timed step as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -405,6 +414,8 @@ def main():
     if rank == 0:
         clocks.start()
     ms, launches, o = timed(step_resident, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(o, args.dump_outputs, R)
     ms_e2e, _, _ = timed(step_e2e, args.steps)
     if rank == 0:
         clocks.stop_flag.set()
@@ -439,14 +450,12 @@ def main():
     k_flops = 2.0 * MAC_SDF_HEAD * P
     achieved = k_flops / (k_ms * 1e-3) / 1e12
     passes = 3 if use_tc else 1
-    # dram__bytes_read.sum + dram__bytes_write.sum of this launch, read from the committed ncu --set full capture
-    traffic_bytes, traffic_src = ncu_traffic_bytes() if use_tc else (None, None)
     roofline = {
-        "bound": "tensor", "achieved": achieved, "peak": burst, "unit": "TFLOP/s", "frac": achieved / burst, "traffic": traffic_bytes, "traffic_source": traffic_src,
+        "bound": "tensor", "achieved": achieved, "peak": burst, "unit": "TFLOP/s", "frac": achieved / burst, "traffic": None, "traffic_source": "not measured",
         "algorithmic_bytes": 16.0 * P,
         "kernel": "SDF-net launch of one sampler round (262144 x 128 points, sdf head only: 0.918 MFLOP/point algorithmic)",
-        "ms_per_launch": k_ms, "peak_source": f"MEASURED_PEAKS.json bf16_tflops ({how}, burst: kernel timed alone)",
-        "mma_mode": "tcgen05 kind::f16, fp16 hi/lo split x3 passes (fp32-level operands, fp32 accumulate)" if use_tc else "fp32 FFMA on CUDA cores (no tensor pipe)",
+        "ms_per_launch": k_ms, "peak_source": f"{how} (burst: kernel timed alone)",
+        "mma_mode": "wgmma m64n256k16 f16, fp16 hi/lo split x3 passes (fp32-level operands, fp32 accumulate)" if use_tc else "fp32 FFMA on CUDA cores (no tensor pipe)",
         "frac_of_mode_peak": achieved / (burst / passes) if use_tc else None,
         "whole_step_tflops": world * flops_per_ray(max(iters)) * R * args.steps / (ms * 1e-3) / 1e12,
         "whole_step_frac_of_sustained": world * flops_per_ray(max(iters)) * R * args.steps / (ms * 1e-3) / 1e12 / (sustained * world),
@@ -487,7 +496,7 @@ def main():
         ctx.check()
         extras["configs[2]_two_hands_object_rays_per_s"] = world * R * 2 / (e0.elapsed_time(e1) * 1e-3)
         extras["configs[2]_sampler_rounds"] = [int(x) for x in o3["sampler_iters"].tolist()]
-        extras["note"] = "per-rank measurements x world; same 512x512 frame, beta 0.03; background nets on tcgen05"
+        extras["note"] = "per-rank measurements x world; same 512x512 frame, beta 0.03; background nets on the tensor cores (wgmma)"
     if rank != 0:
         if dist is not None:
             dist.destroy_process_group()
@@ -502,8 +511,8 @@ def main():
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": "configs[1]: right hand + rigid object, 512x512 frame per step per GPU, 128 samples/ray (N_eval 128, N 64, extra 32), beta 0.03",
                    "nodes": list(NODES), "rays_per_step_per_gpu": R, "sampler_rounds": iters, "parallelism": f"rays/frames sharded x{world}, no collective",
-                   "l2": "per-step working set 3.3 GB of samples >> 126 MB L2 (inputs larger than L2)",
-                   "mlp_mode": "tcgen05 fp16-split x3" if use_tc else "fp32 CUDA cores"},
+                   "l2": "per-step working set 3.3 GB of samples >> 50 MB L2 (inputs larger than L2)",
+                   "mlp_mode": "wgmma fp16-split x3" if use_tc else "fp32 CUDA cores"},
         "e2e": {"value": e2e_value, "unit": "rays/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": launches,
         "clocks": clocks.summary(),

@@ -1,7 +1,7 @@
 """ctypes binding of libhold_b200.so (include/hold_b200.h).
 
 PyTorch is used for device memory and streams only; every arithmetic step of the path runs in the
-library's sm_100a kernels.  There is no fallback: if the library is missing or no B200 is visible the
+library's sm_90a kernels.  There is no fallback: if the library is missing or no H100 is visible the
 import of the product path raises.
 """
 from __future__ import annotations
@@ -193,4 +193,4 @@ def mlp_weights(sd: dict, n_layers: int) -> tuple[MlpWeights, list]:
         w.weight_g[l] = g.data_ptr() if g is not None else None
         w.bias[l] = b.data_ptr()
     return w, keep
-TC_READY = True  # tcgen05 MLP path built into libhold_b200.so
+TC_READY = True  # tensor-core (wgmma) MLP path built into libhold_b200.so

@@ -179,8 +179,8 @@ int hold_ctx_create(hold_ctx** out, int device) {
   HOLD_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   HOLD_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("device %d is sm_%d%d; hold_b200 is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device %d is sm_%d%d; hold_b200 is built for sm_90a only", device, prop.major, prop.minor);
     return HOLD_E_CUDA;
   }
   hold_ctx* ctx = new (std::nothrow) hold_ctx();
@@ -251,7 +251,7 @@ int hold_ctx_check(hold_ctx* ctx, void* stream) {
   HOLD_CUDA(cudaMemcpyAsync(&h, ctx->dev_err, sizeof(int), cudaMemcpyDeviceToHost, s));
   HOLD_CUDA(cudaStreamSynchronize(s));
   if (h != 0) HOLD_CUDA(cudaMemsetAsync(ctx->dev_err, 0, sizeof(int), s));
-  if (h & 0x100) { set_error("tcgen05 pipeline wait timed out (tag %d): protocol error in k_mlp_tc", (h >> 12) & 0xF); return HOLD_E_STATE; }
+  if (h & 0x100) { set_error("tensor-core pipeline wait timed out (tag %d): protocol error in k_mlp_tc", (h >> 12) & 0xF); return HOLD_E_STATE; }
   if (h & kErrRayMiss) { set_error("a ray misses the scene bounding sphere (engine/ray_sampler.py:15-18)"); return HOLD_E_RAY_MISSES_SPHERE; }
   if (h & kErrNonFinite) { set_error("non-finite value (singular transform)"); return HOLD_E_NONFINITE; }
   return HOLD_OK;
@@ -629,7 +629,7 @@ int hold_shade(hold_ctx* ctx, int node, int R, int B, int S, const float* cam_lo
   const int rays_per_chunk = max(1, min(rpf, max_pts / S));
   const size_t cp = (size_t)rays_per_chunk * S;
   // canonical points of the WHOLE call in one launch (full grid, one vertex-group setup per block instead of one per 1 Mi-point
-  // chunk: the per-chunk launches of round 1 ran at 0.57 waves); the MLP stages below are chunked for their 1 GB feature buffer
+  // chunk, whose launches fill only part of a wave); the MLP stages below are chunked for their 1 GB feature buffer
   float* xc_all = out->canonical_pts;
   if (xc_all == nullptr) {
     WS(WS_XC, float, (size_t)R * S * 3, xc_ws);
@@ -970,7 +970,7 @@ int hold_mc_emit(hold_ctx* ctx, int n0, int n1, int n2, const float* vol, float 
   return HOLD_OK;
 }
 
-/* measurement hook (not in the public header): key 2 = accumulator compensation c of the tcgen05 SDF chains (profiles/r02_tc_accumulator_bias.md) */
+/* measurement hook (not in the public header): key 2 = accumulator compensation c of the tensor-core SDF chains (tools/exp_r2b.py) */
 int hold_debug_set(hold_ctx* ctx, int key, int value) {
   if (!ctx) return HOLD_E_BADARG;
   if (key == 2) ctx->tc_acc_comp = value;
@@ -1121,7 +1121,7 @@ int hold_linear(hold_ctx* ctx, int node, int mat, int P, const float* A, int lda
     int rc = check_node(ctx, node, true);
     if (rc) return rc;
     NodeState& ns = ctx->nodes[node];
-    HOLD_REQUIRE(ns.tc != nullptr, "hold_linear needs the packed tcgen05 weight images (hold_node_set_weights)");
+    HOLD_REQUIRE(ns.tc != nullptr, "hold_linear needs the packed tensor-core weight images (hold_node_set_weights)");
     if (mat >= 0 && mat <= 8) { img = ns.tc->sdf_img[mat]; bias = ns.sdf.bias[mat]; nst = ns.tc->sdf_nst[mat]; kmax = (mat == 0) ? kEmbed : 256; nmax = ns.sdf.N[mat]; }
     else if (mat >= 16 && mat <= 24) { img = ns.tc->sdf_imgT[mat - 16]; kmax = (mat - 16 == 3) ? kHidden - kEmbed : 256; nmax = (mat == 16) ? kEmbed : 256; }
     else if (mat >= 32 && mat <= 35) { img = ns.tc->rgb_img[mat - 32]; bias = ns.rgb.bias[mat - 32]; nst = ns.tc->rgb_nst[mat - 32]; kmax = (mat == 32) ? 320 : 256; }
@@ -1144,8 +1144,8 @@ int hold_wgrad(hold_ctx* ctx, int P, const float* D, int ldd, int N, const float
   WgArgs a;
   a.P = P, a.N = N, a.K = K, a.ldd = ldd, a.lda = lda, a.ldo = ldo, a.D = D, a.A = A, a.d_scale = d_scale, a.a_scale = a_scale;
   a.out = out, a.err = ctx->dev_err;
-  const int slabs = ceil_div(P, kWgPts);
-  k_wgrad_tc<<<min(slabs, ctx->sm_count), kWgThreads, kWgSmem, s>>>(a);
+  const int slabs = ceil_div(P, kWgPts), nblk = ceil_div(N, kWgRowsD);
+  k_wgrad_tc<<<dim3(max(1, min(slabs, ctx->sm_count / nblk)), nblk), kWgThreads, kWgSmem, s>>>(a);
   HOLD_LAUNCH_CHECK(ctx);
   return HOLD_OK;
 }

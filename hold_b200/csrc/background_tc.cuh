@@ -1,7 +1,7 @@
-// tcgen05 path of the background nets (hold_bg_set_weights(..., HOLD_MLP_TC); HOLD_MLP_FP32 = the exact-fp32 CUDA-core path of background.cuh):
+// Tensor-core path of the background nets (hold_bg_set_weights(..., HOLD_MLP_TC); HOLD_MLP_FP32 = the exact-fp32 CUDA-core path of background.cuh):
 // k_mlp_tc<MLP_BG_SDF> = inverted-sphere point + PE-10 + frame code -> 8 x 256 Softplus(100) layers (skip at 4) -> sdf head
 // + 256-d feature; k_mlp_tc<MLP_BG_RGB> = [feature | view PE-4 | frame code] (315) -> 128 ReLU -> 3 sigmoid.  Same fp16
-// hi/lo split arithmetic as the foreground nets (first hardware run in round 2: parity with the fp32 path green).
+// hi/lo split arithmetic as the foreground nets (tests/test_gpu_background.py holds it to the fp32 path).
 #pragma once
 #include "background.cuh"
 #include "mlp_tc.cuh"
@@ -37,7 +37,7 @@ static void tc_bg_free(TcBg*& t) {
 static int tc_bg_init() {
   cudaError_t e = cudaFuncSetAttribute(k_mlp_tc<MLP_BG_SDF>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<MLP_BG_SDF>::kSmemBytes);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_mlp_tc<MLP_BG_RGB>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<MLP_BG_RGB>::kSmemBytes);
-  if (e != cudaSuccess) { set_error("tcgen05 background kernel attribute: %s", cudaGetErrorString(e)); return HOLD_E_CUDA; }
+  if (e != cudaSuccess) { set_error("tensor-core background kernel attribute: %s", cudaGetErrorString(e)); return HOLD_E_CUDA; }
   return HOLD_OK;
 }
 

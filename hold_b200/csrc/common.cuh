@@ -1,4 +1,4 @@
-// hold_b200 — shared declarations for the sm_100a kernels behind include/hold_b200.h
+// hold_b200 — shared declarations for the sm_90a kernels behind include/hold_b200.h
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -41,8 +41,8 @@ struct PackedMlp {           // fp32 CUDA-core layout: Wt[l] is [Kpad][Npad] (k-
   float* b_last = nullptr;
 };
 
-struct TcMlp;  // tcgen05 packing, mlp_tc.cuh
-struct TcBg;   // tcgen05 packing of the background nets, background_tc.cuh
+struct TcMlp;  // tensor-core packing, mlp_tc.cuh
+struct TcBg;   // tensor-core packing of the background nets, background_tc.cuh
 
 struct NodeState {
   bool configured = false, has_weights = false, has_rig = false;
@@ -66,7 +66,7 @@ struct Buffer {
 
 struct hold_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   hold::NodeState nodes[HOLD_MAX_NODES];
   int* dev_err = nullptr;
   int64_t launches = 0;
@@ -124,7 +124,7 @@ __device__ inline float laplace_density(float s, float beta) {
   return (1.0f / beta) * (0.5f + 0.5f * sg * expm1f(-fabsf(s) / beta));
 }
 
-// ---- NeRF++ background geometry (model/renderables/background.py), shared by background.cuh and the tcgen05 variant
+// ---- NeRF++ background geometry (model/renderables/background.py), shared by background.cuh and the tensor-core variant
 constexpr int kBgN = 32;        // N_samples_inverse_sphere
 constexpr int kBgEmbed = 84;    // 4 + 4*2*10
 constexpr int kBgFrame = 32;    // dim_frame_encoding

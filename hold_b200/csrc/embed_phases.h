@@ -1,4 +1,4 @@
-// The Fourier embedding of the tcgen05 chains (engine/embedders.py:48-51), as host/device functions: the kernels (mlp_tc.cuh) inline
+// The Fourier embedding of the tensor-core chains (engine/embedders.py:48-51), as host/device functions: the kernels (mlp_tc.cuh) inline
 // them; tests/test_cpu_embed.py runs the same code on the host against the oracle's embedder (value and derivative, 3- and 4-d
 // points, BARF weights, every group offset the kernels use).
 #pragma once
@@ -37,9 +37,8 @@ HOLD_EHD float emb_ldg(const float* p) {
 
 // sin and cos of x for |x| < ~1e4 (the embeddings' arguments are coordinate * 2^k, k <= 9, |coordinate| <= a few): two-constant
 // Cody-Waite reduction by pi/2 with FMAs, Taylor kernels on [-pi/4, pi/4]; max abs error 7.1e-8 over the range used (libm's sinf:
-// 3.3e-8; the pin against the oracle's torch.sin is the stage tests' 1e-4).  No slow path, no calls: eight of these run
-// interleaved per epilogue hand-off.  (The libm sinf / cosf calls this replaces sat behind a non-inlined function and cost ~500
-// clocks EACH, serially, on the critical path of every tile's prologue and skip layer: 13 % of the sdf-only kernel.)
+// 3.3e-8; the pin against the oracle's torch.sin is the stage tests' 1e-4).  No slow path, no calls, so that several of these
+// interleave in the tile prologue and the skip-layer epilogue (libm's sinf / cosf sit behind a non-inlined call and run serially).
 HOLD_EHD void sincos_cw(float x, float& s, float& c) {
   const float k = rintf(x * 0.63661977236758134f);
   float r = fmaf(k, -1.57079637050628662109375f, x);
@@ -60,25 +59,25 @@ HOLD_EHD void sincos_cw(float x, float& s, float& c) {
   c = ((q + 1) & 2) ? -cc : cc;
 }
 
-// Eight consecutive elements e0 .. e0+7 of the Fourier embedding (engine/embedders.py:48-51: [x, sin(2^0 x), cos(2^0 x), sin(2^1 x),
+// NE consecutive elements e0 .. e0+NE-1 of the Fourier embedding (engine/embedders.py:48-51: [x, sin(2^0 x), cos(2^0 x), sin(2^1 x),
 // ...], D coordinates per point, n_embed elements) or, DERIV, of its derivative w.r.t. the element's own coordinate.  Branch-free:
-// the eight sin/cos chains interleave (per-element branches serialise them: ~3 k clocks per hand-off on the tile's critical path).
+// the NE sin/cos chains interleave (per-element branches would serialise them on the tile's critical path).
 // ew: optional per-element weights (BarfEmbedder).  Returns the mask of elements that exist (0 <= e < n_embed); v[i] is finite
 // garbage elsewhere.
-template <int D, bool DERIV>
-HOLD_EHD uint32_t embed8_inl(int e0, int n_embed, float x0, float x1, float x2, float x3, const float* __restrict__ ew,
-                                               float (&v)[8]) {
+template <int D, bool DERIV, int NE>
+HOLD_EHD uint32_t embedn_inl(int e0, int n_embed, float x0, float x1, float x2, float x3, const float* __restrict__ ew,
+                             float (&v)[NE]) {
   uint32_t okm = 0;
-  float w[8];
+  float w[NE];
   if (ew != nullptr) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) w[i] = emb_ldg(ew + (e0 + i < 0 ? 0 : (e0 + i > n_embed - 1 ? n_embed - 1 : e0 + i)));
+    for (int i = 0; i < NE; ++i) w[i] = emb_ldg(ew + (e0 + i < 0 ? 0 : (e0 + i > n_embed - 1 ? n_embed - 1 : e0 + i)));
   } else {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) w[i] = 1.f;
+    for (int i = 0; i < NE; ++i) w[i] = 1.f;
   }
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
+  for (int i = 0; i < NE; ++i) {
     const int e = e0 + i;
     const bool ok = (unsigned)e < (unsigned)n_embed;
     const int ec = ok ? e : 0;

@@ -1,6 +1,6 @@
 // SURVEY §8f rank 3 — training-only loss targets: signed distance of canonical sample points to a closed triangle mesh,
 // i.e. what compute_mano_cano_sdf / check_off_in_surface_points_cano_mesh (engine/volsdf_utils.py:172-217) obtain from
-// kaolin v0.10.0 (absent from /root/reference): `kaolin.metrics.trianglemesh.point_to_mesh_distance` = squared distance
+// kaolin v0.10.0 (absent from the reference's tree): `kaolin.metrics.trianglemesh.point_to_mesh_distance` = squared distance
 // to the nearest face (brute force over faces) and `kaolin.ops.mesh.check_sign` = inside/outside of the watertight
 // mesh.  Distance: closest point on a triangle by Voronoi regions (Ericson, Real-Time Collision Detection 5.1.5).
 // Sign: generalized winding number, sum of the faces' signed solid angles (van Oosterom & Strackee 1983) / 4 pi — for a

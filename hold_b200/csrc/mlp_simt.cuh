@@ -11,7 +11,7 @@
 
 namespace hold {
 
-enum { MLP_SDF_ONLY = 0, MLP_SDF_JVP = 1, MLP_COLOR = 2, MLP_SDF_REV = 3, MLP_BG_SDF = 4, MLP_BG_RGB = 5, MLP_LINEAR = 6 };  // 4, 5, 6: tcgen05 only
+enum { MLP_SDF_ONLY = 0, MLP_SDF_JVP = 1, MLP_COLOR = 2, MLP_SDF_REV = 3, MLP_BG_SDF = 4, MLP_BG_RGB = 5, MLP_LINEAR = 6 };  // 4, 5, 6: tensor cores only
 
 constexpr int kTileRows = 64;
 constexpr int kActLd = 308;   // >= 304 (colour-net input 302 -> 304) + 4

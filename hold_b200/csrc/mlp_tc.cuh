@@ -1,24 +1,22 @@
-// tcgen05 (5th-gen tensor core) fused MLP chains — HOLD_MLP_TC.
+// Tensor-core fused MLP chains on Hopper (sm_90a wgmma) — HOLD_MLP_TC.
 //
 // One persistent CTA per SM walks 128-row tiles through the whole layer chain:
-//   * warp 0           : bulk-async (TMA engine) copies of pre-swizzled fp16 weight chunks L2 -> smem ring
-//   * warp 1           : tcgen05.mma issuer; D[128 x 256] fp32 accumulators in TMEM, ping-pong per layer
-//                        (both walk their loops warp-uniformly and elect the issuing lane, see elect_one())
-//   * warps 2..17      : epilogue — tcgen05.ld the accumulator in 32-column hand-offs, bias + activation in fp32,
-//                        split into fp16 hi/lo and write the next layer's A operand (SW128 K-major) to smem;
-//                        chunk-level mbarriers let layer l+1's MMAs start while layer l's epilogue is running.
+//   * warps 0..7 : two consumer warpgroups, each owning 64 rows of the tile.  Per layer a warpgroup issues wgmma.mma_async
+//                  m64n256k16 over the layer's weight stages into a [64 x 256] fp32 accumulator held in its registers (128 per
+//                  thread), then runs the epilogue on those registers: bias + activation in fp32, split into fp16 hi/lo, and
+//                  write the next layer's A operand (SW128 K-major) for its own 64 rows back to shared memory.  The two
+//                  warpgroups share only the weight ring, so one warpgroup's epilogue overlaps the other's MMAs.
+//   * warp 8     : (of a third warpgroup that hands its registers to the consumers through setmaxnreg) bulk-async (TMA engine) copies of pre-swizzled fp16 weight chunks L2 -> smem ring, mbarrier handshake
+//                  (full: transaction count; empty: one arrival per consumer warp once its wgmma group has read the stage).
 // Arithmetic: every fp32 operand x is split x = hi + lo (fp16 each: 11 + 11 mantissa bits) and each product is
-// three MMAs (hi*hi + lo*hi + hi*lo, fp32 accumulate) — ~2^-21 relative per product (measured 2.5e-7 on a
-// 256-term dot, i.e. fp32-GEMM level), with an absolute floor of ~3e-8 where lo goes subnormal.  This is what the
-// 1e-4 parity bar needs: an sdf error eps reaches the density as eps/beta^2 (beta down to 1e-2), so plain bf16
-// (2^-9) and even a bf16 split (2^-16, measured 83 % of pixels within 1e-4) do not meet it (SURVEY §7 "hard
-// parts").  Range: |x| must stay below 65504 (activations/weights here are O(1e-3..1e2)).  The sdf / rgb heads (1 resp. 3 output
-// rows) are fp32 dot products in the epilogue.  Gradients: reverse mode in the same kernel (MODE MLP_SDF_REV): the forward
-// epilogues stash softplus'(z_l) as unorm16 (512 KB per CTA: 76 MB for the grid, L2-resident; quantisation step 1.5e-5 moves
-// the gradient by <= 1.2e-5 of its scale, tests/test_cpu_stash_quant.py), the backward layers run over transposed weight images.
+// three MMAs (hi*hi + lo*hi + hi*lo, fp32 accumulate) — ~2^-21 relative per product (fp32-GEMM level), with an absolute floor
+// of ~3e-8 where lo goes subnormal.  This is what the 1e-4 parity bar needs: an sdf error eps reaches the density as eps/beta^2
+// (beta down to 1e-2), so plain bf16 (2^-9) and even a bf16 split (2^-16) do not meet it (SURVEY §7 "hard parts").  Range: |x|
+// must stay below 65504 (activations/weights here are O(1e-3..1e2)).  The sdf / rgb heads (1 resp. 3 output rows) are fp32 dot
+// products in the epilogue.  Gradients: reverse mode in the same kernel (MODE MLP_SDF_REV): the forward epilogues stash
+// softplus'(z_l) as unorm16 (512 KB per CTA, L2-resident; quantisation step 1.5e-5 moves the gradient by <= 1.2e-5 of its
+// scale, tests/test_cpu_stash_quant.py), the backward layers run over transposed weight images.
 // Embeddings (tile prologue, skip layer) are inlined branch-free sin/cos (sincos_cw).
-// Round-2 A/B on hardware (profiles/r02_variants.md) retired the other variants (base-2-domain epilogue, rebuilt 16-column
-// epilogue, CTA-pair kernels, forward-mode gradient): none beat this kernel at equal error.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -31,18 +29,18 @@ namespace hold {
 constexpr int kTcRows = 128;
 constexpr int kTcStageBytes = 32768;      // one weight stage: [256 n x 32 k] fp16 hi (16 KB) + lo (16 KB)
 constexpr int kTcAChunkBytes = 16384;     // one A chunk: [128 rows x 64 k] fp16
-constexpr int kTcThreads = 192;
 // Power-of-two operand scaling (exact): fp16 operands are fed to the tensor core as A * 2^6 and W * 2^10 so that
 // the LOW halves of the hi/lo split stay in fp16's normal range for |a| >= 2e-3, |w| >= 1.2e-4 (unscaled, the low
-// half of every |x| < 0.125 is subnormal; measured: the split then gains only 2x over bf16).  The accumulator is
-// rescaled by 2^-16 in the epilogue's bias FMA.  Range: |a| < 1023, |w| < 64.
+// half of every |x| < 0.125 is subnormal and the split gains only 2x over bf16).  The accumulator is rescaled by 2^-16 in
+// the epilogue's bias FMA.  Range: |a| < 1023, |w| < 64.
 constexpr float kTcScaleA = 64.0f, kTcScaleW = 1024.0f, kTcUnscale = 1.0f / (64.0f * 1024.0f);
-// Accumulator-truncation compensation of the Softplus chains.  tcgen05.mma adds into its fp32 accumulator with truncation (round
-// toward zero), not round-to-nearest: measured against float64 on hardware (profiles/r02_tc_accumulator_bias.md) every layer of
-// 48 accumulations (K = 256 x 3 passes) comes out SHRUNK by ~12 x 2^-24 relative — a bias, identical for the hand and object
-// nets and for perturbed weights (zero crossing of the mean sdf error at c = 11.1 / 11.0 / 12.4 / 12.9).  Undoing it in the
-// epilogue's unscale multiply (free) cuts the sdf error 5-8x (5.99e-6 -> 9.5e-7 of the sdf scale), which is what the Laplace
-// density needs at small beta (error amplification 1 / (2 beta^2), engine/density.py:21-26).
+// Accumulator-truncation compensation of the Softplus chains: the tensor core adds into its fp32 accumulator with truncation
+// (round toward zero), not round-to-nearest, so every layer of 48 accumulations (K = 256 x 3 passes) comes out shrunk by a few
+// units of 2^-24 relative — a bias, not noise.  Undoing it in the epilogue's unscale multiply (free) lowers the sdf error, which
+// is what the Laplace density needs at small beta (error amplification 1 / (2 beta^2), engine/density.py:21-26).  Measured on the
+// H100 against float64 (tools/exp_r2b.py section 1, hand and object nets, reference init and perturbed): the mean sdf error crosses
+// zero at c = 11.0 .. 12.9, and c = 12 lowers the max sdf error 4-7x against c = 0 (DESIGN.md §3.1).  hold_debug_set key 2
+// overrides it for such measurements.
 constexpr int kTcAccComp = 12;
 
 constexpr int kTcMaxSteps = 17;
@@ -70,7 +68,7 @@ struct TcMlp {
 struct TcArgs {
   int P, n_layers;
   TcLayer L[kTcMaxSteps];
-  uint16_t* sig;  // reverse mode: per-CTA stash of softplus'(z_l) as unorm16, [grid][8][128][256]
+  uint16_t* sig;  // reverse mode: per-CTA stash of softplus'(z_l) as unorm16, [grid][8 layers][128 rows x 256 columns]
   const float* w_last;
   const float* b_last;
   const float* xc;
@@ -89,7 +87,7 @@ struct TcArgs {
   const float* dirs;
   const float* frame_code;
   float r_sphere;
-  float unscale;             // accumulator -> value: kTcUnscale (times the experimental compensation factor, hold_debug_set key 2)
+  float unscale;             // accumulator -> value: kTcUnscale (times the accumulator compensation, hold_debug_set key 2)
   // MLP_LINEAR (hold_linear): C[P, nvalid] = A[P, kvalid] . W^T (+ bias): one layer against one packed image
   const float* lin_in;
   float* lin_out;
@@ -97,7 +95,7 @@ struct TcArgs {
                              // inside the fp16 hi/lo split's range)
   int lda, ldc, kvalid, nvalid;
   int passes;                // MMAs per product: 3 = hi*hi + lo*hi + hi*lo (always, in production); 2 / 1 only through the measurement
-                             // hook hold_debug_set(ctx, 3, n) for the sampler rounds (profiles/r02_sampler_precision.md)
+                             // hook hold_debug_set(ctx, 3, n) for the sampler rounds
 };
 
 // ------------------------------------------------------------------------------------------------ PTX wrappers
@@ -136,38 +134,10 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// generic-proxy st.shared -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// One lane of a fully converged warp.  The single-thread roles (bulk copies, tcgen05.mma / commit) run their loops
-// with ALL lanes and elect the issuing lane per instruction group: with warp-uniform control flow the compiler keeps
-// descriptors and barrier addresses in uniform registers; inside an `if (lane == 0)` region it wraps every UTCHMMA /
-// UTCBAR / UBLKCP in an ELECT + R2UR.BROADCAST + BRA.U.ANY loop (~25 instructions each), which made the issuer
-// thread the bottleneck of the whole kernel (~1 k clk of issue overhead per weight stage).
+// One lane of a fully converged warp: the producer warp walks its loop with ALL lanes (warp-uniform control flow keeps the
+// barrier addresses in uniform registers) and elects the issuing lane per bulk copy.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
   asm volatile(
@@ -177,22 +147,74 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
+// Barrier over one warpgroup (named barrier `id`, 128 threads) that also returns whether `v` holds in every thread: the
+// warpgroup leaves a pipeline together (wgmma is warpgroup-collective, so a partial exit would stall the rest).
+__device__ __forceinline__ bool wg_all(bool v, int id) {
+  uint32_t r;
+  asm volatile(
+      "{\n\t.reg .pred p, q;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "bar.red.and.pred q, %2, 128, p;\n\t"
+      "selp.u32 %0, 1, 0, q;\n\t}"
+      : "=r"(r)
+      : "r"((uint32_t)v), "r"(id)
+      : "memory");
+  return r != 0;
+}
 
-// UMMA shared-memory descriptor, K-major canonical layouts (cute/arch/mma_sm100_desc.hpp semantics):
-// start address >> 4 | LBO (=1, unused for swizzled K-major) | SBO = bytes between 8-row groups | version 1 | layout
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
+// wgmma shared-memory matrix descriptor (sm_90 GMMA format), K-major canonical layouts:
+// start address >> 4 | LBO (=1, unused for swizzled K-major) | SBO = bytes between 8-row groups | layout type (bits 62-63)
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout_type << 61;
+  d |= (uint64_t)layout_type << 62;
   return d;
 }
-constexpr uint32_t kLayoutSW128 = 2, kLayoutSW64 = 4;
-// kind::f16 instruction descriptor: D=f32, A=B=f16 (format 0), both K-major, N=256, M=128
-constexpr uint32_t kIdescF16 = (1u << 4) | (0u << 7) | (0u << 10) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
-constexpr uint32_t kIdescF16N64 = (1u << 4) | (0u << 7) | (0u << 10) | ((64u >> 3) << 17) | ((128u >> 4) << 24);   // the same with N = 64
+constexpr uint32_t kLayoutSW128 = 1, kLayoutSW64 = 2;
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x 256] (+)= A[64 x 16] . B[256 x 16]^T, fp16 operands from shared memory (both K-major), fp32 accumulator in registers.
+// Fragment of D in thread t of the warpgroup (warp w = t / 32, lane): d[4j + 2h + i] = D[16 w + lane / 4 + 8 h][8 j + 2 (lane % 4) + i].
+__device__ __forceinline__ void wgmma_256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accum)
+      : "memory");
+}
 
 // x = hi + lo: hi = fp16(x), lo = fp16(x - hi)
 __device__ __forceinline__ void split8(const float* x, uint4& hi, uint4& lo) {
@@ -207,6 +229,13 @@ __device__ __forceinline__ void split8(const float* x, uint4& hi, uint4& lo) {
   }
   hi = make_uint4(h[0], h[1], h[2], h[3]);
   lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  const __half2 hh = __floats2half2_rn(x0, x1);
+  const float2 hf = __half22float2(hh);
+  const __half2 ll = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+  hi = *reinterpret_cast<const uint32_t*>(&hh);
+  lo = *reinterpret_cast<const uint32_t*>(&ll);
 }
 // byte offset of the 16-byte unit holding k = 8j..8j+7 of row r inside one [128 x 64] SW128 K-major A chunk
 __device__ __forceinline__ uint32_t a_unit_off(int r, int j) {
@@ -238,174 +267,177 @@ __device__ __forceinline__ uint32_t unorm16_pack2(float s0, float s1) {
 __device__ __forceinline__ float unorm16_lo(uint32_t w) { return __uint_as_float(__byte_perm(w, 0x4B000000u, 0x7410)) - 8388608.0f; }
 __device__ __forceinline__ float unorm16_hi(uint32_t w) { return __uint_as_float(__byte_perm(w, 0x4B000000u, 0x7432)) - 8388608.0f; }
 
-// (Measured, profiles/r02_epilogue_experiments.md: making this and the head dot products out-of-line functions behind one
-// shared epilogue body -- to shrink the kernel from 49 KB to 28 KB of code -- was 5 % SLOWER than one specialised body per layer
-// kind with everything inlined: the branchy shared body costs more per hand-off than the instruction cache misses it avoids.)
 struct Embed8 { float v[8]; uint32_t ok; };
 template <int D, bool DERIV>
 __device__ __forceinline__ Embed8 embed8(int e0, int n_embed, float x0, float x1, float x2, float x3, const float* __restrict__ ew) {
   Embed8 r;
-  if (e0 >= n_embed || e0 + 8 <= 0) {   // (warp-uniform) no element of this group exists
+  if (e0 >= n_embed || e0 + 8 <= 0) {   // no element of this group exists
 #pragma unroll
     for (int i = 0; i < 8; ++i) r.v[i] = 0.f;
     r.ok = 0;
     return r;
   }
-  r.ok = embed8_inl<D, DERIV>(e0, n_embed, x0, x1, x2, x3, ew, r.v);
+  r.ok = embedn_inl<D, DERIV>(e0, n_embed, x0, x1, x2, x3, ew, r.v);
   return r;
 }
-// the 1- or 3-row output heads: fp32 dot products of 8 activation columns with the head rows
-__device__ __forceinline__ float head_dot8(const float* __restrict__ w, float o0, float o1, float o2, float o3, float o4, float o5, float o6, float o7) {
-  const float4 w0 = __ldg(reinterpret_cast<const float4*>(w)), w1 = __ldg(reinterpret_cast<const float4*>(w) + 1);
-  return (o0 * w0.x + o1 * w0.y + o2 * w0.z + o3 * w0.w) + (o4 * w1.x + o5 * w1.y + o6 * w1.z + o7 * w1.w);
+// elements e0, e0 + 1 of the embedding (one accumulator column pair of the epilogue); returns the mask of those that exist
+template <int D, bool DERIV>
+__device__ __forceinline__ uint32_t embed2(int e0, int n_embed, const float (&pt)[4], const float* __restrict__ ew, float (&v)[2]) {
+  if (e0 >= n_embed || e0 + 2 <= 0) {
+    v[0] = v[1] = 0.f;
+    return 0;
+  }
+  return embedn_inl<D, DERIV>(e0, n_embed, pt[0], pt[1], pt[2], pt[3], ew, v);
 }
 
-constexpr int kTcW = 4;                        // epilogue warps per TMEM lane quarter
-constexpr int kTcChunk = 32;                   // accumulator columns per epilogue->MMA hand-off (= one weight stage of k)
-constexpr int kTcCW = kTcChunk / kTcW;         // accumulator columns per warp per chunk
-constexpr int kTcEpiWarps = 4 * kTcW;
-constexpr int kTcEpiThreads = 32 * kTcEpiWarps;
-constexpr int kTcThreadsTotal = 64 + kTcEpiThreads;
-
-__device__ __forceinline__ void tc_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-// One arrival per epilogue WARP on the hand-off barrier: every lane orders its own st.shared against the async
-// proxy, the warp converges, lane 0 arrives.
-__device__ __forceinline__ void handoff_arrive(uint32_t bar, int lane) {
-#if !defined(HOLD_TC_EXP) || (HOLD_TC_EXP != 3 && HOLD_TC_EXP != 6)
-  fence_proxy_async();
-#endif
-  tc_fence_before();
-  __syncwarp();
-  if (lane == 0) mbar_arrive(bar);
-}
-__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, %0;" ::"n"(kTcEpiThreads) : "memory"); }
+constexpr int kTcConsumers = 256;                     // two warpgroups: warps 0..7
+constexpr int kTcThreadsTotal = kTcConsumers + 128;   // + the producer warpgroup (warp 8 issues the copies, 9..11 exit at once)
+// registers per thread after the warpgroups' setmaxnreg: producer 40, consumers 232 (128 x 40 + 256 x 232 <= 64 K)
+constexpr int kTcProducerRegs = 40, kTcConsumerRegs = 232;
 
 template <int MODE>
 struct TcCfg {
   static constexpr bool kColorLike = (MODE == MLP_COLOR || MODE == MLP_BG_RGB);   // ReLU chain with a 3-row sigmoid head
   static constexpr bool kWide = kColorLike || MODE == MLP_LINEAR;                  // first operand up to 320 wide
   static constexpr int kAChunks = kWide ? 5 : 4;   // 64-wide SW128 A chunks in smem
-  static constexpr int kHandoffs = 2 * kAChunks;                 // 32-wide epilogue->MMA hand-offs
   static constexpr int kStages = kWide ? 2 : 3;
   static constexpr int kSmemA = 2 * kAChunks * kTcAChunkBytes;
   static constexpr int kSmemW = kStages * kTcStageBytes;
-  static constexpr int kSmemBytes = kSmemA + kSmemW + 256 + 1024;  // + barriers (<= 2*3 + 10 + 8, 8 B each) + 1 KB alignment slack
+  static constexpr int kSmemBytes = kSmemA + kSmemW + 256 + 1024;  // + barriers (2 x 3, 8 B each) and the abort flag + 1 KB alignment slack
 };
 
-// Per-thread state of an epilogue warp (kept in registers: every user is force-inlined).
-struct EpiState {
-  uint32_t bAReady, bDFull, t_lane;
-  uint8_t* a_row;        // generic pointer to this thread's row inside A chunk 0 (hi part)
-  uint32_t u0, lo_off;   // byte offset of the thread's 16-byte unit for even hand-offs (odd: u0 ^ 64); hi -> lo part distance
-  int sub, lane, p;
-  bool valid;
-  float px, py, pz, pw;
-  float head0, head1, head2;
-  uint32_t d_par;        // bit b = parity to wait for on d_full[b]
+// Weight ring and A operand of one consumer warpgroup.
+struct Pipe {
+  uint32_t a_hi, a_lo;     // this warpgroup's 64 rows of A chunk 0 (hi / lo part), shared-space addresses
+  uint32_t sW, bWFull, bWEmpty;
+  uint32_t stage, phase;
+  int ns, lane, bar_id;
   volatile int* abort_flag;
 };
 
-// One layer of a forward chain (every mode but the reverse-mode gradient and hold_linear): wait for the accumulator, then 8
-// hand-offs of 32 columns; per hand-off this warp turns its 8 columns into the next layer's fp16 hi/lo operand.
+// All MMAs of layer l for this warpgroup: acc = A . W_l^T over the layer's k stages (PASSES MMAs per k16 step).  A stage is released
+// to the producer when the wgmma group that read it has completed (one group in flight behind the one just issued).  PASSES is a
+// template parameter so that no branch sits between the wgmmas on the accumulator (ptxas would serialise them with extra
+// warpgroup.arrive instructions).
+template <int PASSES>
+__device__ __forceinline__ bool mma_layer_p(const TcArgs& a, Pipe& P, const int l, float (&acc)[128]) {
+  const int nst = a.L[l].nst;
+  uint32_t prev = 0;
+  for (int s = 0; s < nst; ++s) {
+    const bool got = mbar_wait(P.bWFull + 8 * P.stage, P.phase, a.err, 3, P.abort_flag);
+    if (!wg_all(got, P.bar_id)) {
+      wgmma_wait<0>();
+      return false;
+    }
+    const uint32_t wb = P.sW + P.stage * kTcStageBytes;
+    const int c = s >> 1;  // 64-wide A chunk holding this 32-k stage
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint32_t koff = (uint32_t)(((s & 1) * 2 + j) * 32);  // bytes inside the 128-byte A row
+      const uint64_t ahi = gmma_desc(P.a_hi + c * kTcAChunkBytes + koff, 1024, kLayoutSW128);
+      const uint64_t alo = gmma_desc(P.a_lo + c * kTcAChunkBytes + koff, 1024, kLayoutSW128);
+      const uint64_t whi = gmma_desc(wb + j * 32, 512, kLayoutSW64);
+      const uint64_t wlo = gmma_desc(wb + 16384 + j * 32, 512, kLayoutSW64);
+      wgmma_256(acc, ahi, whi, (s | j) != 0);
+      if (PASSES >= 2) wgmma_256(acc, alo, whi, 1);
+      if (PASSES >= 3) wgmma_256(acc, ahi, wlo, 1);
+    }
+    wgmma_commit();
+    if (s > 0) {
+      wgmma_wait<1>();
+      __syncwarp();
+      if (P.lane == 0) mbar_arrive(P.bWEmpty + 8 * prev);
+    }
+    prev = P.stage;
+    if (++P.stage == (uint32_t)P.ns) { P.stage = 0; P.phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  __syncwarp();
+  if (P.lane == 0) mbar_arrive(P.bWEmpty + 8 * prev);
+  return true;
+}
+__device__ __forceinline__ bool mma_layer(const TcArgs& a, Pipe& P, const int l, float (&acc)[128]) {
+  if (a.passes >= 3) return mma_layer_p<3>(a, P, l, acc);
+  return (a.passes == 2) ? mma_layer_p<2>(a, P, l, acc) : mma_layer_p<1>(a, P, l, acc);
+}
+
+// Per-thread view of the accumulator fragment: rows r[0] and r[1] = r[0] + 8 of the tile, columns 8 j + 2 q + {0, 1}, j = 0..31.
+struct Frag {
+  uint8_t* a_row[2];     // generic pointer to row r[h] inside A chunk 0 (hi part), plus the thread's 4-byte slot
+  int r7[2];             // r[h] & 7 (the SW128 swizzle of the row)
+  uint32_t lo_off;       // hi -> lo part distance
+  int q;
+  int p[2];
+  bool valid[2];
+  float pt[2][4];        // the rows' points (embedding inputs of the skip columns)
+  float head[2][3];
+  float gz[2];           // reverse mode: d sdf / d z (head[h][1], head[h][2] hold d/dx, d/dy)
+};
+
+// two fp16 hi/lo pairs of the next layer's operand for accumulator columns c0 = 8 j + 2 q, c0 + 1 of row h
+__device__ __forceinline__ void frag_store_a(const Frag& F, int h, int j, float o0, float o1) {
+  uint32_t hi, lo;
+  split2(o0, o1, hi, lo);
+  uint8_t* dst = F.a_row[h] + (j >> 3) * kTcAChunkBytes + (((j & 7) ^ F.r7[h]) << 4);
+  *reinterpret_cast<uint32_t*>(dst) = hi;
+  *reinterpret_cast<uint32_t*>(dst + F.lo_off) = lo;
+}
+
+// One layer of a forward chain (every mode but the reverse-mode gradient and hold_linear), on the accumulator in registers:
 //   HEAD : the 1- (sdf) or 3-row (colour) output head is accumulated from this layer's activations (fp32 dot products)
 //   WRITE: the activations are the next MMA's operand (false on the chain's last MMA layer)
 //   FEAT : the layer's outputs are the 256-d feature vector (no activation, stored to global memory)
 //   SKIP : output columns >= a.L[l].N are the point's embedding (the skip connection into the next layer, shape_net.py:116-119)
-// One specialised body per layer kind (see the note at embed8).  a.L[l].bias is pre-multiplied by kTcScaleA unless FEAT
-// (TcMlp::bias_s).  The hand-off loop is unrolled by two with explicit ping-pong registers for the prefetched bias and
-// accumulator columns (a rotating prefetch costs 8 MOVs per hand-off).  The accumulator arrives in four 64-column quarters.
+// One specialised body per layer kind.  a.L[l].bias is pre-multiplied by kTcScaleA unless FEAT (TcMlp::bias_s).
 template <int MODE, bool HEAD, bool WRITE, bool FEAT, bool SKIP>
-__device__ __forceinline__ bool epi_layer(const TcArgs& a, EpiState& E, const int l) {
+__device__ __forceinline__ void epi_layer(const TcArgs& a, Frag& F, const int l, const float (&acc)[128]) {
   constexpr bool kColorLike = (MODE == MLP_COLOR || MODE == MLP_BG_RGB);
   const int N = a.L[l].N;
-  const float* bias = a.L[l].bias + E.sub * 8;
-  float4 nb[2][2];
-  nb[0][0] = __ldg(reinterpret_cast<const float4*>(bias));      // issued before the wait
-  nb[0][1] = __ldg(reinterpret_cast<const float4*>(bias) + 1);
-#if defined(HOLD_TC_EXP) && HOLD_TC_EXP == 7
-  const bool rec = blockIdx.x == 0 && (E.p / kTcRows) == 2 * (int)gridDim.x && E.sub == 0 && (threadIdx.x & 127) == 64 && a.sig != nullptr;
-  uint32_t* rbuf = reinterpret_cast<uint32_t*>(a.sig) + l * 16;
-  if (rec) rbuf[0] = (uint32_t)clock();
-#endif
-  const uint32_t dbar = E.bDFull + 32 * (l & 1), dpar = (E.d_par >> (l & 1)) & 1;   // four quarter barriers, one parity (each completes once per layer)
-  if (!mbar_wait(dbar, dpar, a.err, 4, E.abort_flag)) return false;
-#if defined(HOLD_TC_EXP) && HOLD_TC_EXP == 7
-  if (rec) rbuf[1] = (uint32_t)clock();
-#endif
-  E.d_par ^= (1u << (l & 1));
-  tc_fence_after();
-  const uint32_t t_col = E.t_lane + (uint32_t)((l & 1) * 256 + E.sub * 8);
+  const float* bias = a.L[l].bias;
   const float us = FEAT ? a.unscale : a.unscale * kTcScaleA;
-  uint32_t raw[2][8];
-  tc_ld8(t_col, raw[0]);
-#if defined(HOLD_TC_EXP) && HOLD_TC_EXP == 12   // timing experiment: four hand-offs per loop iteration
-#pragma unroll 2
-#else
-#pragma unroll 1
-#endif
-  for (int c = 0; c < 4; ++c) {
 #pragma unroll
-    for (int hb = 0; hb < 2; ++hb) {
-      const int h = 2 * c + hb;
-      const int n0 = h * 32 + E.sub * 8;
-      if (hb == 0 || c < 3) {   // the next hand-off's bias: an un-prefetched load is a cache round trip on every hand-off's critical path
-        nb[hb ^ 1][0] = __ldg(reinterpret_cast<const float4*>(bias + 32 * (h + 1)));
-        nb[hb ^ 1][1] = __ldg(reinterpret_cast<const float4*>(bias + 32 * (h + 1)) + 1);
+  for (int j = 0; j < 32; ++j) {
+    const int c0 = 8 * j + 2 * F.q;
+    const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + c0));
+    float2 w0, w1, w2;
+    if (HEAD) {
+      w0 = __ldg(reinterpret_cast<const float2*>(a.w_last + c0));
+      if (kColorLike) {
+        w1 = __ldg(reinterpret_cast<const float2*>(a.w_last + 256 + c0));
+        w2 = __ldg(reinterpret_cast<const float2*>(a.w_last + 512 + c0));
       }
-      const float bv[8] = {nb[hb][0].x, nb[hb][0].y, nb[hb][0].z, nb[hb][0].w, nb[hb][1].x, nb[hb][1].y, nb[hb][1].z, nb[hb][1].w};
-      tc_wait_ld();
-      if (hb == 1 && c < 3) {   // the next hand-off opens the accumulator's next 64-column quarter
-        if (!mbar_wait(dbar + 8 * (c + 1), dpar, a.err, 4, E.abort_flag)) return false;
-        tc_fence_after();
-      }
-      if (hb == 0 || c < 3) tc_ld8(t_col + (uint32_t)((h + 1) * 32), raw[hb ^ 1]);   // prefetch the next hand-off's columns
-      float out[8];
+    }
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        // accumulator -> pre-activation times kTcScaleA (undo the weight scaling, add the scaled bias); out[] is the next
-        // layer's operand, i.e. the activation times kTcScaleA (FEAT: the plain output)
-        const float zs = fmaf(__uint_as_float(raw[hb][i]), us, bv[i]);
-        float e;
-        out[i] = FEAT ? zs : (kColorLike ? fmaxf(zs, 0.f) : softplus100_scaled(zs, e));
-      }
-      if (SKIP && n0 + 8 > N) {  // skip connection: embedding columns of layer 3's output
-        const Embed8 ev = (MODE == MLP_BG_SDF) ? embed8<4, false>(n0 - N, kBgEmbed, E.px, E.py, E.pz, E.pw, nullptr)
-                                               : embed8<3, false>(n0 - N, kEmbed, E.px, E.py, E.pz, 0.f, a.embed_w);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) out[i] = (n0 + i >= N) ? (((ev.ok >> i) & 1u) ? kTcScaleA * ev.v[i] : 0.f) : out[i];
+    for (int h = 0; h < 2; ++h) {
+      // accumulator -> pre-activation times kTcScaleA (undo the weight scaling, add the scaled bias); o is the next layer's operand,
+      // i.e. the activation times kTcScaleA (FEAT: the plain output)
+      const float z0 = fmaf(acc[4 * j + 2 * h], us, bv.x), z1 = fmaf(acc[4 * j + 2 * h + 1], us, bv.y);
+      float o0, o1, e;
+      if (FEAT) o0 = z0, o1 = z1;
+      else if (kColorLike) o0 = fmaxf(z0, 0.f), o1 = fmaxf(z1, 0.f);
+      else o0 = softplus100_scaled(z0, e), o1 = softplus100_scaled(z1, e);
+      if (SKIP && 8 * j + 8 > N) {  // skip connection: embedding columns of layer 3's output
+        float ev[2];
+        const uint32_t ok = (MODE == MLP_BG_SDF) ? embed2<4, false>(c0 - N, kBgEmbed, F.pt[h], nullptr, ev)
+                                                 : embed2<3, false>(c0 - N, kEmbed, F.pt[h], a.embed_w, ev);
+        o0 = (c0 >= N) ? ((ok & 1u) ? kTcScaleA * ev[0] : 0.f) : o0;
+        o1 = (c0 + 1 >= N) ? ((ok & 2u) ? kTcScaleA * ev[1] : 0.f) : o1;
       }
       if (HEAD) {
-        E.head0 += head_dot8(a.w_last + n0, out[0], out[1], out[2], out[3], out[4], out[5], out[6], out[7]);
+        F.head[h][0] += o0 * w0.x + o1 * w0.y;
         if (kColorLike) {
-          E.head1 += head_dot8(a.w_last + 256 + n0, out[0], out[1], out[2], out[3], out[4], out[5], out[6], out[7]);
-          E.head2 += head_dot8(a.w_last + 512 + n0, out[0], out[1], out[2], out[3], out[4], out[5], out[6], out[7]);
+          F.head[h][1] += o0 * w1.x + o1 * w1.y;
+          F.head[h][2] += o0 * w2.x + o1 * w2.y;
         }
       }
       if (FEAT) {
-        if (E.valid) {
-          float4* dst = reinterpret_cast<float4*>(a.feat + (size_t)E.p * kFeat + n0);
-          dst[0] = make_float4(out[0], out[1], out[2], out[3]);
-          dst[1] = make_float4(out[4], out[5], out[6], out[7]);
-        }
+        if (F.valid[h]) *reinterpret_cast<float2*>(a.feat + (size_t)F.p[h] * kFeat + c0) = make_float2(o0, o1);
       } else if (WRITE) {
-        uint4 hi, lo;
-        split8(out, hi, lo);
-        uint8_t* dst = E.a_row + c * kTcAChunkBytes + (hb ? (E.u0 ^ 64u) : E.u0);
-        *reinterpret_cast<uint4*>(dst) = hi;
-        *reinterpret_cast<uint4*>(dst + E.lo_off) = lo;
-        handoff_arrive(E.bAReady + 16 * c + 8 * hb, E.lane);
-#if defined(HOLD_TC_EXP) && HOLD_TC_EXP == 7
-        if (rec) rbuf[2 + h] = (uint32_t)clock();
-#endif
+        frag_store_a(F, h, j, o0, o1);
       }
     }
   }
-  return true;
 }
 
 // Reverse-mode chain (MODE MLP_SDF_REV), one step = one accumulator: d sdf/d z_7 = w_sdf * s_7;  d sdf/d z_{l-1} = (g_l . W_l) * s_{l-1};
@@ -414,535 +446,379 @@ __device__ __forceinline__ bool epi_layer(const TcArgs& a, EpiState& E, const in
 //   KIND 1: the feature layer (st = 8): writes the 256-d feature, seeds g_7 = w_sdf * s_7
 //   KIND 2: backward layer l = 16 - st: operand of the next step = acc * s_{l-1};  SPEC 1: l = 4 (its columns >= 217 are d sdf/d embed)
 //   KIND 3: st = 16: d sdf / d embed through layer 0's input, no operand
-// One specialised body per (KIND, SPEC), same structure as epi_layer (ping-pong registers for the prefetched bias / accumulator
-// columns; the stash words are read two hand-offs ahead into the slot that was just consumed).  The monolithic step body this
-// replaces issued 223 instructions per 8-column hand-off (ncu) against 107 in the forward-only chain.
-// Stash: s_l as unorm16, written and later read by the SAME thread (row, 8 columns per hand-off), L2 only (.cg): 512 KB per CTA.
-struct RevState {
-  uint16_t* sig;         // this thread's row of the CTA's stash, [8 layers][128 rows][256]
-  float gz;              // d sdf / d z (head1 / head2 of the EpiState hold d/dx, d/dy)
-};
-
+// Stash: s_l as unorm16 pairs, written and later read by the SAME thread (its fragment), L2 only (.cg), laid out so that a warp's
+// 32 words of one (layer, column pair, row half) are contiguous: 512 KB per CTA.
 template <int KIND, int SPEC>
-__device__ __forceinline__ bool rev_step(const TcArgs& a, EpiState& E, RevState& R, const int st) {
+__device__ __forceinline__ void rev_step(const TcArgs& a, Frag& F, uint32_t* sigw, const int st, const float (&acc)[128]) {
   constexpr float kInvQ = 1.0f / 65535.0f;
-  constexpr int kRowStride = kTcRows * 256;
   const int l = (st <= 8) ? st : 16 - st;
-  const float* bias = (KIND <= 1) ? a.L[st].bias + E.sub * 8 : nullptr;
-  // stash row read by this step: s_7 for the feature layer's seed, s_{l-1} for backward layer l
-  const uint16_t* srow = (KIND == 1) ? R.sig + (size_t)7 * kRowStride + E.sub * 8 : ((KIND == 2) ? R.sig + (size_t)(l - 1) * kRowStride + E.sub * 8 : nullptr);
-  float4 nb[2][2];
-  uint4 sq[2];
-  if (KIND <= 1) {
-    nb[0][0] = __ldg(reinterpret_cast<const float4*>(bias));
-    nb[0][1] = __ldg(reinterpret_cast<const float4*>(bias) + 1);
-  }
-  if (KIND == 1 || KIND == 2) {
-    sq[0] = __ldcg(reinterpret_cast<const uint4*>(srow));
-    sq[1] = __ldcg(reinterpret_cast<const uint4*>(srow + 32));
-  }
-  const uint32_t dbar = E.bDFull + 32 * (st & 1), dpar = (E.d_par >> (st & 1)) & 1;
-  if (!mbar_wait(dbar, dpar, a.err, 4, E.abort_flag)) return false;
-  E.d_par ^= (1u << (st & 1));
-  tc_fence_after();
-  const uint32_t t_col = E.t_lane + (uint32_t)((st & 1) * 256 + E.sub * 8);
+  const float* bias = (KIND <= 1) ? a.L[st].bias : nullptr;
+  // stash layer read by this step: s_7 for the feature layer's seed, s_{l-1} for backward layer l
+  const int sl = (KIND == 1) ? 7 : l - 1;
   const float us = (KIND == 0) ? a.unscale * kTcScaleA : a.unscale;   // forward layers work on kTcScaleA * z (bias pre-scaled)
-  uint32_t raw[2][8];
-  tc_ld8(t_col, raw[0]);
-#if defined(HOLD_TC_EXP) && HOLD_TC_EXP == 12   // timing experiment: four hand-offs per loop iteration
-#pragma unroll 2
-#else
-#pragma unroll 1
-#endif
-  for (int c = 0; c < 4; ++c) {
 #pragma unroll
-    for (int hb = 0; hb < 2; ++hb) {
-      const int h = 2 * c + hb;
-      const int n0 = h * 32 + E.sub * 8;
-      if (KIND <= 1 && (hb == 0 || c < 3)) {
-        nb[hb ^ 1][0] = __ldg(reinterpret_cast<const float4*>(bias + 32 * (h + 1)));
-        nb[hb ^ 1][1] = __ldg(reinterpret_cast<const float4*>(bias + 32 * (h + 1)) + 1);
-      }
-      const float bv[8] = {nb[hb][0].x, nb[hb][0].y, nb[hb][0].z, nb[hb][0].w, nb[hb][1].x, nb[hb][1].y, nb[hb][1].z, nb[hb][1].w};
-      const uint4 sqv = sq[hb];
-      if ((KIND == 1 || KIND == 2) && c < 3) sq[hb] = __ldcg(reinterpret_cast<const uint4*>(srow + 32 * (h + 2)));   // two hand-offs ahead
-      tc_wait_ld();
-      if (hb == 1 && c < 3) {   // the next hand-off opens the accumulator's next 64-column quarter
-        if (!mbar_wait(dbar + 8 * (c + 1), dpar, a.err, 4, E.abort_flag)) return false;
-        tc_fence_after();
-      }
-      if (hb == 0 || c < 3) tc_ld8(t_col + (uint32_t)((h + 1) * 32), raw[hb ^ 1]);
-      float out[8];
+  for (int j = 0; j < 32; ++j) {
+    const int c0 = 8 * j + 2 * F.q;
+    float2 bv = make_float2(0.f, 0.f), wl = make_float2(0.f, 0.f);
+    if (KIND <= 1) bv = __ldg(reinterpret_cast<const float2*>(bias + c0));
+    if ((KIND == 0 && SPEC == 2) || KIND == 1) wl = __ldg(reinterpret_cast<const float2*>(a.w_last + c0));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float r0 = acc[4 * j + 2 * h], r1 = acc[4 * j + 2 * h + 1];
+      float o0 = 0.f, o1 = 0.f;
       if (KIND == 0) {
-        float sg[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float e;
-          const float zs = fmaf(__uint_as_float(raw[hb][i]), us, bv[i]);
-          out[i] = softplus100_scaled(zs, e);
-          const float r = mufu_rcp(1.0f + e);
-          sg[i] = (zs >= 0.f) ? r : e * r;
+        float e0, e1;
+        const float z0 = fmaf(r0, us, bv.x), z1 = fmaf(r1, us, bv.y);
+        o0 = softplus100_scaled(z0, e0), o1 = softplus100_scaled(z1, e1);
+        const float q0 = mufu_rcp(1.0f + e0), q1 = mufu_rcp(1.0f + e1);
+        __stcg(sigw + ((l * 32 + j) * 2 + h) * kTcConsumers, unorm16_pack2((z0 >= 0.f) ? q0 : e0 * q0, (z1 >= 0.f) ? q1 : e1 * q1));
+        if (SPEC == 1 && 8 * j + 8 > 217) {
+          float ev[2];
+          const uint32_t ok = embed2<3, false>(c0 - 217, kEmbed, F.pt[h], a.embed_w, ev);
+          o0 = (ok & 1u) ? kTcScaleA * ev[0] : o0;
+          o1 = (ok & 2u) ? kTcScaleA * ev[1] : o1;
         }
-        __stcg(reinterpret_cast<uint4*>(R.sig + (size_t)l * kRowStride + n0),
-               make_uint4(unorm16_pack2(sg[0], sg[1]), unorm16_pack2(sg[2], sg[3]), unorm16_pack2(sg[4], sg[5]), unorm16_pack2(sg[6], sg[7])));
-        if (SPEC == 1 && n0 + 8 > 217) {
-          const Embed8 ev = embed8<3, false>(n0 - 217, kEmbed, E.px, E.py, E.pz, 0.f, a.embed_w);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) out[i] = ((ev.ok >> i) & 1u) ? kTcScaleA * ev.v[i] : out[i];
-        }
-        if (SPEC == 2) E.head0 += head_dot8(a.w_last + n0, out[0], out[1], out[2], out[3], out[4], out[5], out[6], out[7]);
+        if (SPEC == 2) F.head[h][0] += o0 * wl.x + o1 * wl.y;
       } else {
-        // softplus' of this hand-off's 8 columns (times 65535; the scale is folded below)
-        const float sv[8] = {unorm16_lo(sqv.x), unorm16_hi(sqv.x), unorm16_lo(sqv.y), unorm16_hi(sqv.y),
-                             unorm16_lo(sqv.z), unorm16_hi(sqv.z), unorm16_lo(sqv.w), unorm16_hi(sqv.w)};
+        // softplus' of these 2 columns (times 65535; the scale is folded below)
+        const uint32_t sq = (KIND == 3) ? 0u : __ldcg(sigw + ((sl * 32 + j) * 2 + h) * kTcConsumers);
+        const float s0 = unorm16_lo(sq), s1 = unorm16_hi(sq);
         if (KIND == 1) {
-          if (E.valid) {   // the 256-d feature vector: written once, read once by the colour net -> streaming stores
-            float f[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) f[i] = fmaf(__uint_as_float(raw[hb][i]), us, bv[i]);
-            float4* dst = reinterpret_cast<float4*>(a.feat + (size_t)E.p * kFeat + n0);
-            __stcs(dst, make_float4(f[0], f[1], f[2], f[3]));
-            __stcs(dst + 1, make_float4(f[4], f[5], f[6], f[7]));
+          if (F.valid[h]) {   // the 256-d feature vector: written once, read once by the colour net -> streaming stores
+            __stcs(reinterpret_cast<float2*>(a.feat + (size_t)F.p[h] * kFeat + c0), make_float2(fmaf(r0, us, bv.x), fmaf(r1, us, bv.y)));
           }
-          const float4 w0 = __ldg(reinterpret_cast<const float4*>(a.w_last + n0));
-          const float4 w1 = __ldg(reinterpret_cast<const float4*>(a.w_last + n0) + 1);
-          const float wv[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
           // g_7 = w_sdf * s_7, times the operand scale
-#pragma unroll
-          for (int i = 0; i < 8; ++i) out[i] = (kTcScaleA * kInvQ) * wv[i] * sv[i];
+          o0 = (kTcScaleA * kInvQ) * wl.x * s0, o1 = (kTcScaleA * kInvQ) * wl.y * s1;
         } else {
           if (KIND == 2) {   // operand of the next backward layer: (acc * unscale) * s_{l-1}, times the operand scale (one constant)
             const float k2 = us * (kTcScaleA * kInvQ);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) out[i] = (__uint_as_float(raw[hb][i]) * k2) * sv[i];
+            o0 = (r0 * k2) * s0, o1 = (r1 * k2) * s1;
           }
-          if ((KIND == 2 && SPEC == 1 && n0 + 8 > 217) || (KIND == 3 && n0 < 40)) {  // columns that are d sdf / d embed
-            const int e0 = (KIND == 2) ? n0 - 217 : n0;
-            float acc[8];
+          if ((KIND == 2 && SPEC == 1 && 8 * j + 8 > 217) || (KIND == 3 && 8 * j < 40)) {  // columns that are d sdf / d embed
+            const int e0 = (KIND == 2) ? c0 - 217 : c0;
+            float dv[2];
+            const uint32_t ok = embed2<3, true>(e0, kEmbed, F.pt[h], a.embed_w, dv);
+            const float rr[2] = {r0 * us, r1 * us};
 #pragma unroll
-            for (int i = 0; i < 8; ++i) acc[i] = __uint_as_float(raw[hb][i]) * us;
-            const Embed8 dv = embed8<3, true>(e0, kEmbed, E.px, E.py, E.pz, 0.f, a.embed_w);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
+            for (int i = 0; i < 2; ++i) {
               const int ec = max(e0 + i, 0), d = ec - 3 * ((ec * 171) >> 9);
-              const bool ok = (dv.ok >> i) & 1u;
-              const float je = ok ? acc[i] * dv.v[i] : 0.f;
-              E.head1 += (d == 0) ? je : 0.f;
-              E.head2 += (d == 1) ? je : 0.f;
-              R.gz += (d == 2) ? je : 0.f;
-              if (KIND == 2) out[i] = ok ? 0.f : out[i];
+              const bool okc = (ok >> i) & 1u;
+              const float je = okc ? rr[i] * dv[i] : 0.f;
+              F.head[h][1] += (d == 0) ? je : 0.f;
+              F.head[h][2] += (d == 1) ? je : 0.f;
+              F.gz[h] += (d == 2) ? je : 0.f;
+              if (KIND == 2 && okc) (i == 0 ? o0 : o1) = 0.f;
             }
           }
         }
       }
-      if (KIND != 3) {
-        uint4 hi, lo;
-        split8(out, hi, lo);
-        uint8_t* dst = E.a_row + c * kTcAChunkBytes + (hb ? (E.u0 ^ 64u) : E.u0);
-        *reinterpret_cast<uint4*>(dst) = hi;
-        *reinterpret_cast<uint4*>(dst + E.lo_off) = lo;
-        handoff_arrive(E.bAReady + 16 * c + 8 * hb, E.lane);
-      }
+      if (KIND != 3) frag_store_a(F, h, j, o0, o1);
     }
   }
-  return true;
+}
+
+// Tile prologue of one consumer warpgroup: the layer-0 A operand of its 64 rows, in 8-column units (2 threads per row).
+__device__ __forceinline__ void store_unit(uint8_t* gA_hi, uint8_t* gA_lo, int row, int u, const float (&x)[8]) {
+  uint4 hi, lo;
+  split8(x, hi, lo);
+  const uint32_t off = (uint32_t)((u >> 3) * kTcAChunkBytes) + a_unit_off(row, u & 7);
+  *reinterpret_cast<uint4*>(gA_hi + off) = hi;
+  *reinterpret_cast<uint4*>(gA_lo + off) = lo;
+}
+
+template <int MODE>
+__device__ __forceinline__ void prologue(const TcArgs& a, uint8_t* gA_hi, uint8_t* gA_lo, const int row, const int p, const int half) {
+  constexpr bool kColorLike = (MODE == MLP_COLOR || MODE == MLP_BG_RGB);
+  const bool valid = p < a.P;
+  if (MODE == MLP_LINEAR) {
+    // rows of a [P, lda] fp32 matrix, columns [0, kvalid) (zero padded to the image's K), optionally divided by *in_scale
+    const float isc = (a.in_scale != nullptr) ? kTcScaleA / __ldg(a.in_scale) : kTcScaleA;
+    const float* src = a.lin_in + (size_t)p * a.lda;
+    const int nu = a.L[0].nst * 4;
+#pragma unroll 1
+    for (int u = half; u < nu; u += 2) {
+      const int k0 = 8 * u;
+      float x[8];
+      if (valid && k0 + 8 <= a.kvalid) {
+        const float4 f0 = __ldg(reinterpret_cast<const float4*>(src + k0)), f1 = __ldg(reinterpret_cast<const float4*>(src + k0) + 1);
+        x[0] = f0.x, x[1] = f0.y, x[2] = f0.z, x[3] = f0.w, x[4] = f1.x, x[5] = f1.y, x[6] = f1.z, x[7] = f1.w;
+      } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) x[i] = (valid && k0 + i < a.kvalid) ? __ldg(src + k0 + i) : 0.f;
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) x[i] *= isc;
+      store_unit(gA_hi, gA_lo, row, u, x);
+    }
+  } else if (MODE == MLP_BG_SDF) {
+    // inverted-sphere point of sample p % 32 of ray p / 32 (background.py:63-68,102-135), PE-10 + frame code: 116 -> 128
+    float p4[4] = {0.f, 0.f, 0.f, 0.f};
+    if (valid) {
+      const int ray = p / kBgN;
+      const float o[3] = {a.cam[3 * ray], a.cam[3 * ray + 1], a.cam[3 * ray + 2]};
+      const float d[3] = {a.dirs[3 * ray], a.dirs[3 * ray + 1], a.dirs[3 * ray + 2]};
+      depth2pts_outside(o, d, bg_depth(p % kBgN, a.r_sphere), a.r_sphere, p4);
+    }
+    const int b = valid ? p / a.pts_per_frame : 0;
+#pragma unroll 1
+    for (int u = half; u < 16; u += 2) {
+      float x[8];
+      const int e0 = 8 * u;
+      const Embed8 ev = embed8<4, false>(e0, kBgEmbed, p4[0], p4[1], p4[2], p4[3], nullptr);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int e = e0 + i;
+        float v = ((ev.ok >> i) & 1u) ? ev.v[i] : 0.f;
+        if (e >= kBgEmbed && e < kBgEmbed + kBgFrame) v = a.frame_code[b * kBgFrame + e - kBgEmbed];
+        x[i] = kTcScaleA * v;
+      }
+      store_unit(gA_hi, gA_lo, row, u, x);
+    }
+  } else if (!kColorLike) {
+    float px = 0.f, py = 0.f, pz = 0.f;
+    if (valid) { px = a.xc[3 * (size_t)p], py = a.xc[3 * (size_t)p + 1], pz = a.xc[3 * (size_t)p + 2]; }
+#pragma unroll 1
+    for (int u = half; u < 8; u += 2) {
+      float x[8];
+      const Embed8 ev = embed8<3, false>(8 * u, kEmbed, px, py, pz, 0.f, a.embed_w);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) x[i] = ((ev.ok >> i) & 1u) ? kTcScaleA * ev.v[i] : 0.f;
+      store_unit(gA_hi, gA_lo, row, u, x);
+    }
+  } else {
+    const int b = valid ? p / a.pts_per_frame : 0;
+#pragma unroll 1
+    for (int u = half; u < 40; u += 2) {
+      float x[8];
+      const int k0 = 8 * u;
+      if (k0 < kFeat) {
+        if (valid) {
+          const float4 f0 = *reinterpret_cast<const float4*>(a.feat + (size_t)p * kFeat + k0);
+          const float4 f1 = *reinterpret_cast<const float4*>(a.feat + (size_t)p * kFeat + k0 + 4);
+          x[0] = f0.x, x[1] = f0.y, x[2] = f0.z, x[3] = f0.w, x[4] = f1.x, x[5] = f1.y, x[6] = f1.z, x[7] = f1.w;
+        } else {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) x[i] = 0.f;
+        }
+      } else {
+        Embed8 ev;
+        ev.ok = 0;
+        if (MODE == MLP_BG_RGB) {
+          const int ray = valid ? p / kBgN : 0;
+          ev = embed8<3, false>(k0 - kFeat, kBgView, a.dirs[3 * ray], a.dirs[3 * ray + 1], a.dirs[3 * ray + 2], 0.f, nullptr);
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int e = k0 + i - kFeat;  // [x_c(3), n(3), pose_embed(8), time_code(32)]; background: [view PE-4 (27), frame code (32)]
+          float v = 0.f;
+          if (MODE == MLP_BG_RGB) {
+            if (valid) {
+              if ((ev.ok >> i) & 1u) v = ev.v[i];
+              else if (e >= kBgView && e < kBgView + kBgFrame) v = a.frame_code[b * kBgFrame + e - kBgView];
+            }
+          } else if (valid) {
+            if (e < 3) v = a.xc[3 * (size_t)p + e];
+            else if (e < 6) v = a.normal[3 * (size_t)p + e - 3];
+            else if (e < 14) v = (a.pose_embed != nullptr) ? a.pose_embed[b * 8 + e - 6] : 0.f;
+            else if (e < a.k0 - kFeat) v = a.time_code[b * 32 + e - 14];
+          }
+          x[i] = v;
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) x[i] *= kTcScaleA;
+      store_unit(gA_hi, gA_lo, row, u, x);
+    }
+  }
+}
+
+// sum over the 4 threads (lane % 4) that share a fragment row: fixed order, so the result does not depend on scheduling
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
 }
 
 template <int MODE>
 __global__ void __launch_bounds__(kTcThreadsTotal, 1) k_mlp_tc(TcArgs a) {
-  static_assert(MODE == MLP_SDF_ONLY || MODE == MLP_SDF_REV || MODE == MLP_COLOR || MODE == MLP_BG_SDF || MODE == MLP_BG_RGB || MODE == MLP_LINEAR, "chains built on tcgen05");
+  static_assert(MODE == MLP_SDF_ONLY || MODE == MLP_SDF_REV || MODE == MLP_COLOR || MODE == MLP_BG_SDF || MODE == MLP_BG_RGB || MODE == MLP_LINEAR, "chains built on wgmma");
   if (a.st != nullptr && a.st->done) return;
   using Cfg = TcCfg<MODE>;
   constexpr bool kColorLike = Cfg::kColorLike;
-  constexpr int NA = Cfg::kAChunks, NS = Cfg::kStages, NHO = Cfg::kHandoffs;
-  constexpr int PPT = kTcRows;
+  constexpr int NA = Cfg::kAChunks, NS = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sA_hi = base, sA_lo = base + NA * kTcAChunkBytes, sW = base + Cfg::kSmemA;
   const uint32_t sBar = sW + Cfg::kSmemW;
-  const uint32_t bWFull = sBar, bWEmpty = sBar + 8 * NS, bAReady = sBar + 16 * NS, bDFull = bAReady + 8 * NHO;
-  const uint32_t sTmemPtr = bDFull + 64, sAbort = bDFull + 68;   // d_full: [2 accumulators][4 column quarters]
+  const uint32_t bWFull = sBar, bWEmpty = sBar + 8 * NS, sAbort = sBar + 16 * NS;
   uint8_t* gen_base = smem_raw + (base - smem_u32(smem_raw));  // generic pointer to `base`
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   volatile int* abort_flag = reinterpret_cast<volatile int*>(gen_base + (sAbort - base));
-  const int n_tiles = ceil_div(a.P, PPT);
+  const int n_tiles = ceil_div(a.P, kTcRows);
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NS; ++i) { mbar_init(bWFull + 8 * i, 1); mbar_init(bWEmpty + 8 * i, 1); }
+    for (int i = 0; i < NS; ++i) { mbar_init(bWFull + 8 * i, 1); mbar_init(bWEmpty + 8 * i, kTcConsumers / 32); }  // empty: one arrival per consumer warp
     *abort_flag = 0;
-    for (int i = 0; i < NHO; ++i) mbar_init(bAReady + 8 * i, kTcEpiWarps);  // one arrival per epilogue warp
-    for (int i = 0; i < 8; ++i) mbar_init(bDFull + 8 * i, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sTmemPtr), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(gen_base + (sTmemPtr - base));
 
-  if (warp == 0) {
+  if (warp >= kTcConsumers / 32) {
     // ============================================================ weight producer (TMA engine, bulk async copies)
-    {
-      uint32_t stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        for (int l = 0; l < a.n_layers; ++l) {
-          const uint8_t* src = a.L[l].wimg;
-          for (int s = 0; s < a.L[l].nst; ++s) {
-            if (!__all_sync(0xffffffffu, mbar_wait(bWEmpty + 8 * stage, phase ^ 1, a.err, 1, abort_flag))) goto tc_done;
-            if (elect_one()) {
-              mbar_expect_tx(bWFull + 8 * stage, kTcStageBytes);
-              bulk_g2s(sW + stage * kTcStageBytes, src + (size_t)s * kTcStageBytes, kTcStageBytes, bWFull + 8 * stage);
-            }
-            __syncwarp();
-            if (++stage == NS) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ============================================================ MMA issuer (whole warp walks the loop, one elected lane issues)
-    {
-      uint32_t stage = 0, phase = 0;
-      uint32_t a_par = 0;  // bit c = parity to wait for on a_ready[c]
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem, 0);
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        for (int l = 0; l < a.n_layers; ++l) {
-          const uint32_t d_tmem = tmem_u + (uint32_t)((l & 1) * 256);
-          const int nst = a.L[l].nst;
-          for (int s = 0; s < nst; ++s) {
-            const int c = s >> 1;  // 64-wide A chunk holding this 32-k stage
-            // hand-off s = columns [32 s, 32 s + 32) of the previous layer's activations
-            if (!__all_sync(0xffffffffu, mbar_wait(bAReady + 8 * s, (a_par >> s) & 1, a.err, 2, abort_flag))) goto tc_done;
-            a_par ^= (1u << s);
-            if (!__all_sync(0xffffffffu, mbar_wait(bWFull + 8 * stage, phase, a.err, 3, abort_flag))) goto tc_done;
-            tc_fence_after();
-#if defined(HOLD_TC_EXP) && HOLD_TC_EXP == 7   // cycle accounting (tools/exp_epilogue.py): stage s of layer l issued at
-            if (blockIdx.x == 0 && tile == 2 * (int)gridDim.x && lane == 0 && a.sig != nullptr) reinterpret_cast<uint32_t*>(a.sig)[256 + l * 16 + s] = (uint32_t)clock();
-#endif
-            const uint32_t wb = sW + stage * kTcStageBytes;
-            const bool el = elect_one();
-            if (s + 1 < nst) {
-#pragma unroll
-              for (int j = 0; j < 2; ++j) {
-                const uint32_t koff = (uint32_t)(((s & 1) * 2 + j) * 32);  // bytes inside the 128-byte A row
-                const uint64_t ahi = umma_desc(sA_hi + c * kTcAChunkBytes + koff, 1024, kLayoutSW128);
-                const uint64_t alo = umma_desc(sA_lo + c * kTcAChunkBytes + koff, 1024, kLayoutSW128);
-                const uint64_t whi = umma_desc(wb + j * 32, 512, kLayoutSW64);
-                const uint64_t wlo = umma_desc(wb + 16384 + j * 32, 512, kLayoutSW64);
-                if (el) {
-                  tc_mma(d_tmem, ahi, whi, kIdescF16, (s | j) != 0);
-                  if (a.passes >= 2) tc_mma(d_tmem, alo, whi, kIdescF16, 1);
-                  if (a.passes >= 3) tc_mma(d_tmem, ahi, wlo, kIdescF16, 1);
-                }
-              }
-            } else {
-              // the layer's LAST k stage goes out as four 64-column quarters, each committed on its own barrier: the epilogue
-              // starts on columns 0..63 while the other three quarters are still in the tensor pipe (measured: the accumulator-
-              // full signal sat ~1.1 k clocks after the last stage's issue, all of it tensor-pipe idle time of the next layer)
-#pragma unroll
-              for (int qn = 0; qn < 4; ++qn) {
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                  const uint32_t koff = (uint32_t)(((s & 1) * 2 + j) * 32);
-                  const uint64_t ahi = umma_desc(sA_hi + c * kTcAChunkBytes + koff, 1024, kLayoutSW128);
-                  const uint64_t alo = umma_desc(sA_lo + c * kTcAChunkBytes + koff, 1024, kLayoutSW128);
-                  const uint64_t whi = umma_desc(wb + qn * 4096 + j * 32, 512, kLayoutSW64);          // rows 64 qn.. of the [256 n x 32 k] image
-                  const uint64_t wlo = umma_desc(wb + 16384 + qn * 4096 + j * 32, 512, kLayoutSW64);
-                  if (el) {
-                    tc_mma(d_tmem + (uint32_t)(64 * qn), ahi, whi, kIdescF16N64, (s | j) != 0);
-                    if (a.passes >= 2) tc_mma(d_tmem + (uint32_t)(64 * qn), alo, whi, kIdescF16N64, 1);
-                    if (a.passes >= 3) tc_mma(d_tmem + (uint32_t)(64 * qn), ahi, wlo, kIdescF16N64, 1);
-                  }
-                }
-                if (el) tc_commit(bDFull + 8 * ((l & 1) * 4 + qn));  // columns [64 qn, 64 qn + 64) of layer l's accumulator complete
-              }
-            }
-            if (el) tc_commit(bWEmpty + 8 * stage);  // frees the weight stage when these MMAs have read it
-            __syncwarp();
-            if (++stage == NS) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else {
-    // ============================================================ epilogue: kTcW warps per TMEM lane quarter; warp
-    // `sub` of a quarter owns columns [sub*CW, (sub+1)*CW) of every 64-column chunk, so chunks complete in order
-    // and layer l+1's MMAs on chunk c start while chunks c+1.. of layer l are still in the epilogue.
-    const int q = warp & 3;
-    const int sub = (warp - 2) >> 2;
-    const int row = q * 32 + lane;
-    const uint32_t t_lane = tmem + ((uint32_t)(q * 32) << 16);
-    uint8_t* gA_hi = gen_base;
-    uint8_t* gA_lo = gen_base + NA * kTcAChunkBytes;
-    float* scratch = reinterpret_cast<float*>(gen_base);  // head partial sums (A region, free at tile end)
-    uint32_t d_par = 0;  // bit b = parity to wait for on d_full[b]
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kTcProducerRegs));
+    if (warp != kTcConsumers / 32) return;
+    uint32_t stage = 0, phase = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      const int p = tile * PPT + row;
-      const bool valid = p < a.P;
-      float px = 0.f, py = 0.f, pz = 0.f, pw = 0.f;
-      // ---------------------------------------------------------- prologue: layer-0 A operand (this warp's columns)
-      if (MODE == MLP_LINEAR) {
-        // rows of a [P, lda] fp32 matrix, columns [0, kvalid) (zero padded to the image's K), optionally divided by *in_scale
-        const float isc = (a.in_scale != nullptr) ? kTcScaleA / __ldg(a.in_scale) : kTcScaleA;
-        const float* src = a.lin_in + (size_t)p * a.lda;
-        const int nst = a.L[0].nst;
-        for (int h = 0; h < nst; ++h) {
-          const int k0 = h * 32 + sub * 8;
-          float x[8];
-          if (valid && k0 + 8 <= a.kvalid) {
-            const float4 f0 = __ldg(reinterpret_cast<const float4*>(src + k0)), f1 = __ldg(reinterpret_cast<const float4*>(src + k0) + 1);
-            x[0] = f0.x, x[1] = f0.y, x[2] = f0.z, x[3] = f0.w, x[4] = f1.x, x[5] = f1.y, x[6] = f1.z, x[7] = f1.w;
-          } else {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) x[i] = (valid && k0 + i < a.kvalid) ? __ldg(src + k0 + i) : 0.f;
+      for (int l = 0; l < a.n_layers; ++l) {
+        const uint8_t* src = a.L[l].wimg;
+        for (int s = 0; s < a.L[l].nst; ++s) {
+          if (!__all_sync(0xffffffffu, mbar_wait(bWEmpty + 8 * stage, phase ^ 1, a.err, 1, abort_flag))) return;
+          if (elect_one()) {
+            mbar_expect_tx(bWFull + 8 * stage, kTcStageBytes);
+            bulk_g2s(sW + stage * kTcStageBytes, src + (size_t)s * kTcStageBytes, kTcStageBytes, bWFull + 8 * stage);
           }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) x[i] *= isc;
-          uint4 hi, lo;
-          split8(x, hi, lo);
-          const int c = h >> 1, j = (h & 1) * 4 + sub;
-          *reinterpret_cast<uint4*>(gA_hi + c * kTcAChunkBytes + a_unit_off(row, j)) = hi;
-          *reinterpret_cast<uint4*>(gA_lo + c * kTcAChunkBytes + a_unit_off(row, j)) = lo;
-          handoff_arrive(bAReady + 8 * h, lane);
+          __syncwarp();
+          if (++stage == NS) { stage = 0; phase ^= 1; }
         }
-      } else if (MODE == MLP_BG_SDF) {
-        // inverted-sphere point of sample p % 32 of ray p / 32 (background.py:63-68,102-135), PE-10 + frame code: 116 -> 128
-        if (valid) {
-          const int ray = p / kBgN;
+      }
+    }
+    return;
+  }
+
+  // ============================================================ consumer warpgroups: MMAs + epilogue on their 64 rows
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTcConsumerRegs));
+  const int wg = warp >> 2, tid = threadIdx.x & 127;
+  uint8_t* gA_hi = gen_base;
+  uint8_t* gA_lo = gen_base + NA * kTcAChunkBytes;
+  Pipe P;
+  P.a_hi = sA_hi + wg * 64 * 128, P.a_lo = sA_lo + wg * 64 * 128;   // 64 rows x 128 bytes of every A chunk
+  P.sW = sW, P.bWFull = bWFull, P.bWEmpty = bWEmpty, P.stage = 0, P.phase = 0, P.ns = NS, P.lane = lane, P.bar_id = 1 + wg;
+  P.abort_flag = abort_flag;
+  Frag F;
+  F.q = lane & 3;
+  F.lo_off = (uint32_t)(NA * kTcAChunkBytes);
+  const int r_frag = wg * 64 + (tid >> 5) * 16 + (lane >> 2);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r_frag + 8 * h;
+    F.r7[h] = r & 7;
+    F.a_row[h] = gA_hi + (r >> 3) * 1024 + (r & 7) * 128 + 4 * F.q;
+  }
+  uint32_t* sigw = (MODE == MLP_SDF_REV) ? reinterpret_cast<uint32_t*>(a.sig) + (size_t)blockIdx.x * (8 * kTcRows * 256 / 2) + threadIdx.x : nullptr;
+  float acc[128];
+
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    // ---------------------------------------------------------- prologue: layer-0 A operand of this warpgroup's rows
+    prologue<MODE>(a, gA_hi, gA_lo, wg * 64 + (tid & 63), tile * kTcRows + wg * 64 + (tid & 63), tid >> 6);
+    fence_proxy_async();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      F.p[h] = tile * kTcRows + r_frag + 8 * h;
+      F.valid[h] = F.p[h] < a.P;
+      F.pt[h][0] = F.pt[h][1] = F.pt[h][2] = F.pt[h][3] = 0.f;
+      F.head[h][0] = F.head[h][1] = F.head[h][2] = 0.f;
+      F.gz[h] = 0.f;
+      if (F.valid[h]) {
+        const size_t p = (size_t)F.p[h];
+        if (MODE == MLP_BG_SDF) {
+          const int ray = (int)(p / kBgN);
           const float o[3] = {a.cam[3 * ray], a.cam[3 * ray + 1], a.cam[3 * ray + 2]};
           const float d[3] = {a.dirs[3 * ray], a.dirs[3 * ray + 1], a.dirs[3 * ray + 2]};
-          float p4[4];
-          depth2pts_outside(o, d, bg_depth(p % kBgN, a.r_sphere), a.r_sphere, p4);
-          px = p4[0], py = p4[1], pz = p4[2], pw = p4[3];
-        }
-        const int b = valid ? p / a.pts_per_frame : 0;
-        for (int h = 0; h < 4; ++h) {
-          float x[8];
-          const int e0 = h * 32 + sub * 8;
-          const Embed8 ev = embed8<4, false>(e0, kBgEmbed, px, py, pz, pw, nullptr);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int e = e0 + i;
-            float v = ((ev.ok >> i) & 1u) ? ev.v[i] : 0.f;
-            if (e >= kBgEmbed && e < kBgEmbed + kBgFrame) v = a.frame_code[b * kBgFrame + e - kBgEmbed];
-            x[i] = kTcScaleA * v;
-          }
-          uint4 hi, lo;
-          split8(x, hi, lo);
-          const int c = h >> 1, j = (h & 1) * 4 + sub;
-          *reinterpret_cast<uint4*>(gA_hi + c * kTcAChunkBytes + a_unit_off(row, j)) = hi;
-          *reinterpret_cast<uint4*>(gA_lo + c * kTcAChunkBytes + a_unit_off(row, j)) = lo;
-          handoff_arrive(bAReady + 8 * h, lane);
-        }
-      } else if (!kColorLike) {
-#if defined(HOLD_TC_EXP) && HOLD_TC_EXP == 7
-        if (blockIdx.x == 0 && tile == 2 * (int)gridDim.x && sub == 0 && (threadIdx.x & 127) == 64 && a.sig != nullptr) reinterpret_cast<uint32_t*>(a.sig)[12] = (uint32_t)clock();
-#endif
-        if (valid) { px = a.xc[3 * (size_t)p], py = a.xc[3 * (size_t)p + 1], pz = a.xc[3 * (size_t)p + 2]; }
-        for (int h = 0; h < 2; ++h) {
-          float x[8];
-          const Embed8 ev = embed8<3, false>(h * 32 + sub * 8, kEmbed, px, py, pz, 0.f, a.embed_w);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) x[i] = ((ev.ok >> i) & 1u) ? kTcScaleA * ev.v[i] : 0.f;
-          uint4 hi, lo;
-          split8(x, hi, lo);
-          const int j = h * 4 + sub;
-          *reinterpret_cast<uint4*>(gA_hi + a_unit_off(row, j)) = hi;
-          *reinterpret_cast<uint4*>(gA_lo + a_unit_off(row, j)) = lo;
-          handoff_arrive(bAReady + 8 * h, lane);
-        }
-      } else {
-        const int b = valid ? p / a.pts_per_frame : 0;
-        for (int h = 0; h < 10; ++h) {
-          float x[8];
-          const int k0 = h * 32 + sub * 8;
-          if (h < 8) {
-            if (valid) {
-              const float4 f0 = *reinterpret_cast<const float4*>(a.feat + (size_t)p * kFeat + k0);
-              const float4 f1 = *reinterpret_cast<const float4*>(a.feat + (size_t)p * kFeat + k0 + 4);
-              x[0] = f0.x, x[1] = f0.y, x[2] = f0.z, x[3] = f0.w, x[4] = f1.x, x[5] = f1.y, x[6] = f1.z, x[7] = f1.w;
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) x[i] = 0.f;
-            }
-          } else {
-            Embed8 ev;
-            ev.ok = 0;
-            if (MODE == MLP_BG_RGB) {
-              const int ray = valid ? p / kBgN : 0;
-              ev = embed8<3, false>(k0 - kFeat, kBgView, a.dirs[3 * ray], a.dirs[3 * ray + 1], a.dirs[3 * ray + 2], 0.f, nullptr);
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int e = k0 + i - kFeat;  // [x_c(3), n(3), pose_embed(8), time_code(32)]; background: [view PE-4 (27), frame code (32)]
-              float v = 0.f;
-              if (MODE == MLP_BG_RGB) {
-                if (valid) {
-                  if ((ev.ok >> i) & 1u) v = ev.v[i];
-                  else if (e >= kBgView && e < kBgView + kBgFrame) v = a.frame_code[b * kBgFrame + e - kBgView];
-                }
-              } else if (valid) {
-                if (e < 3) v = a.xc[3 * (size_t)p + e];
-                else if (e < 6) v = a.normal[3 * (size_t)p + e - 3];
-                else if (e < 14) v = (a.pose_embed != nullptr) ? a.pose_embed[b * 8 + e - 6] : 0.f;
-                else if (e < a.k0 - kFeat) v = a.time_code[b * 32 + e - 14];
-              }
-              x[i] = v;
-            }
-          }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) x[i] *= kTcScaleA;
-          uint4 hi, lo;
-          split8(x, hi, lo);
-          const int c = h >> 1, j = (h & 1) * 4 + sub;
-          *reinterpret_cast<uint4*>(gA_hi + c * kTcAChunkBytes + a_unit_off(row, j)) = hi;
-          *reinterpret_cast<uint4*>(gA_lo + c * kTcAChunkBytes + a_unit_off(row, j)) = lo;
-          handoff_arrive(bAReady + 8 * h, lane);
+          depth2pts_outside(o, d, bg_depth((int)(p % kBgN), a.r_sphere), a.r_sphere, F.pt[h]);
+        } else if (MODE == MLP_SDF_ONLY || MODE == MLP_SDF_REV) {
+          F.pt[h][0] = a.xc[3 * p], F.pt[h][1] = a.xc[3 * p + 1], F.pt[h][2] = a.xc[3 * p + 2];
         }
       }
-      // ---------------------------------------------------------- per-layer epilogues
-      float head0 = 0.f, head1 = 0.f, head2 = 0.f, gz_acc = 0.f;
-      if (MODE == MLP_LINEAR) {
-        // ======== one layer: C = acc * unscale (* in_scale) + bias, fp32 rows of [P, ldc], columns [0, nvalid) ========
-        const float* bias = a.L[0].bias;
-        const float osc = (a.in_scale != nullptr) ? a.unscale * __ldg(a.in_scale) : a.unscale;
-        if (!mbar_wait(bDFull + 24, d_par & 1, a.err, 4, abort_flag)) break;   // the last column quarter: the whole accumulator is complete
-        d_par ^= 1u;
-        tc_fence_after();
-        const uint32_t t_col = t_lane + (uint32_t)(sub * 8);
-        uint32_t raw[8];
-        tc_ld8(t_col, raw);
-        float* dst = a.lin_out + (size_t)p * a.ldc;
-#pragma unroll 2
-        for (int h = 0; h < 8; ++h) {
-          const int n0 = h * 32 + sub * 8;
-          tc_wait_ld();
-          float out[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) out[i] = __uint_as_float(raw[i]) * osc;
-          if (h + 1 < 8) tc_ld8(t_col + (uint32_t)((h + 1) * 32), raw);
-          if (bias != nullptr && n0 < a.nvalid) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) out[i] += (n0 + i < a.nvalid) ? __ldg(bias + n0 + i) : 0.f;
-          }
-          if (valid) {
-            if (n0 + 8 <= a.nvalid) {
-              *reinterpret_cast<float4*>(dst + n0) = make_float4(out[0], out[1], out[2], out[3]);
-              *reinterpret_cast<float4*>(dst + n0 + 4) = make_float4(out[4], out[5], out[6], out[7]);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i)
-                if (n0 + i < a.nvalid) dst[n0 + i] = out[i];
-            }
-          }
-        }
-        tc_fence_before();
-        epi_bar();   // every warp has read its accumulator columns before the next tile's MMAs overwrite them
-        continue;
-      }
-      if (MODE == MLP_SDF_REV) {
-        // ======== reverse-mode gradient: 8 forward layers (stash softplus'), feature layer, 8 backward layers (rev_step) ========
-        {
-          EpiState E;
-          E.bAReady = bAReady, E.bDFull = bDFull, E.t_lane = t_lane;
-          E.a_row = gA_hi + (row >> 3) * 1024 + (row & 7) * 128;
-          E.u0 = (uint32_t)((sub ^ (row & 7)) << 4), E.lo_off = (uint32_t)(NA * kTcAChunkBytes);
-          E.sub = sub, E.lane = lane, E.p = p, E.valid = valid;
-          E.px = px, E.py = py, E.pz = pz, E.pw = 0.f;
-          E.head0 = 0.f, E.head1 = 0.f, E.head2 = 0.f, E.d_par = d_par, E.abort_flag = abort_flag;
-          RevState R;
-          R.sig = a.sig + (size_t)blockIdx.x * (8 * kTcRows * 256) + (size_t)row * 256;
-          R.gz = 0.f;
-          bool ok = true;
-          for (int st = 0; st < 17 && ok; ++st) {
-            if (st < 8) ok = (st == 3) ? rev_step<0, 1>(a, E, R, st) : ((st == 7) ? rev_step<0, 2>(a, E, R, st) : rev_step<0, 0>(a, E, R, st));
-            else if (st == 8) ok = rev_step<1, 0>(a, E, R, st);
-            else if (st < 16) ok = (st == 12) ? rev_step<2, 1>(a, E, R, st) : rev_step<2, 0>(a, E, R, st);
-            else ok = rev_step<3, 0>(a, E, R, st);
-          }
-          d_par = E.d_par, head0 = E.head0, head1 = E.head1, head2 = E.head2, gz_acc = R.gz;
-        }
-        // fixed-order reduction of (sdf head, d/dx, d/dy, d/dz) over the quarter's 4 warps
-        tc_fence_before();
-        scratch[(sub * 4 + 0) * kTcRows + row] = head0;
-        scratch[(sub * 4 + 1) * kTcRows + row] = head1;
-        scratch[(sub * 4 + 2) * kTcRows + row] = head2;
-        scratch[(sub * 4 + 3) * kTcRows + row] = gz_acc;
-        epi_bar();
-        if (sub == 0 && valid) {
-          float hsum[4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            float acc = 0.f;
-#pragma unroll
-            for (int w = 0; w < kTcW; ++w) acc += scratch[(w * 4 + k) * kTcRows + row];
-            hsum[k] = acc;
-          }
-          a.sdf[p] = hsum[0] * (1.0f / kTcScaleA) + a.b_last[0];
-          a.grad[3 * (size_t)p] = hsum[1], a.grad[3 * (size_t)p + 1] = hsum[2], a.grad[3 * (size_t)p + 2] = hsum[3];
-        }
-        epi_bar();
-        continue;
-      }
-      {
-        EpiState E;
-        E.bAReady = bAReady, E.bDFull = bDFull, E.t_lane = t_lane;
-        E.a_row = gA_hi + (row >> 3) * 1024 + (row & 7) * 128;
-        E.u0 = (uint32_t)((sub ^ (row & 7)) << 4), E.lo_off = (uint32_t)(NA * kTcAChunkBytes);
-        E.sub = sub, E.lane = lane, E.p = p, E.valid = valid;
-        E.px = px, E.py = py, E.pz = pz, E.pw = pw;
-        E.head0 = 0.f, E.head1 = 0.f, E.head2 = 0.f, E.d_par = d_par, E.abort_flag = abort_flag;
-        bool ok = true;
-        for (int l = 0; l < a.n_layers && ok; ++l) {
-          const bool head_layer = kColorLike ? (l == a.n_layers - 1) : (l == 7);
-          const bool last_mma = (l == a.n_layers - 1);
-          if (MODE == MLP_BG_SDF && last_mma) ok = epi_layer<MODE, false, false, true, false>(a, E, l);           // the feature rows
-          else if (MODE == MLP_BG_SDF && head_layer) ok = epi_layer<MODE, true, true, false, false>(a, E, l);
-          else if (head_layer) ok = epi_layer<MODE, true, false, false, false>(a, E, l);
-          else if (!kColorLike && l == 3) ok = epi_layer<MODE, false, true, false, true>(a, E, l);
-          else ok = epi_layer<MODE, false, true, false, false>(a, E, l);
-        }
-        d_par = E.d_par, head0 = E.head0, head1 = E.head1, head2 = E.head2;
-        if (!ok) break;
-      }
-      // ---------------------------------------------------------- heads: fixed-order reduction over the quarter's warps
-      // (all MMAs of the tile have completed, so the A region is free to hold the partial sums)
-      tc_fence_before();
-      constexpr int NH = kColorLike ? 3 : 1;
-      scratch[(sub * NH + 0) * kTcRows + row] = head0;
-      if (kColorLike) {
-        scratch[(sub * NH + 1) * kTcRows + row] = head1;
-        scratch[(sub * NH + 2) * kTcRows + row] = head2;
-      }
-      epi_bar();
-      if (sub == 0 && valid) {
-        float h[NH];
-#pragma unroll
-        for (int k = 0; k < NH; ++k) {
-          float acc = 0.f;
-#pragma unroll
-          for (int w = 0; w < kTcW; ++w) acc += scratch[(w * NH + k) * kTcRows + row];
-          h[k] = acc * (1.0f / kTcScaleA);  // the head saw activations times kTcScaleA
-        }
-        if (kColorLike) {
-#pragma unroll
-          for (int k = 0; k < NH; ++k) a.rgb[3 * (size_t)p + k] = 1.0f / (1.0f + __expf(-(h[k] + a.b_last[k])));
-        } else {
-          a.sdf[p] = h[0] + a.b_last[0];
-        }
-      }
-      epi_bar();  // scratch is overwritten by the next tile's prologue
     }
-  }
-tc_done:
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
+    wg_all(true, P.bar_id);   // the operand is complete before any thread of the warpgroup issues the first MMA
+
+    // ---------------------------------------------------------- layers: MMAs, then the epilogue on the accumulator
+    bool ok = true;
+    if (MODE == MLP_LINEAR) {
+      // ======== one layer: C = acc * unscale (* in_scale) + bias, fp32 rows of [P, ldc], columns [0, nvalid) ========
+      ok = mma_layer(a, P, 0, acc);
+      if (!ok) break;
+      const float* bias = a.L[0].bias;
+      const float osc = (a.in_scale != nullptr) ? a.unscale * __ldg(a.in_scale) : a.unscale;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int c0 = 8 * j + 2 * F.q;
+        if (c0 >= a.nvalid) continue;
+        float2 bv = make_float2(0.f, 0.f);
+        if (bias != nullptr) bv = make_float2(__ldg(bias + c0), (c0 + 1 < a.nvalid) ? __ldg(bias + c0 + 1) : 0.f);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!F.valid[h]) continue;
+          float* dst = a.lin_out + (size_t)F.p[h] * a.ldc + c0;
+          const float o0 = fmaf(acc[4 * j + 2 * h], osc, bv.x), o1 = fmaf(acc[4 * j + 2 * h + 1], osc, bv.y);
+          if (c0 + 1 < a.nvalid) *reinterpret_cast<float2*>(dst) = make_float2(o0, o1);
+          else dst[0] = o0;
+        }
+      }
+    } else if (MODE == MLP_SDF_REV) {
+      // ======== reverse-mode gradient: 8 forward layers (stash softplus'), feature layer, 8 backward layers (rev_step) ========
+      for (int st = 0; st < 17; ++st) {
+        ok = mma_layer(a, P, st, acc);
+        if (!ok) break;
+        if (st < 8) {
+          if (st == 3) rev_step<0, 1>(a, F, sigw, st, acc);
+          else if (st == 7) rev_step<0, 2>(a, F, sigw, st, acc);
+          else rev_step<0, 0>(a, F, sigw, st, acc);
+        } else if (st == 8) {
+          rev_step<1, 0>(a, F, sigw, st, acc);
+        } else if (st < 16) {
+          if (st == 12) rev_step<2, 1>(a, F, sigw, st, acc);
+          else rev_step<2, 0>(a, F, sigw, st, acc);
+        } else {
+          rev_step<3, 0>(a, F, sigw, st, acc);
+        }
+        fence_proxy_async();
+        wg_all(true, P.bar_id);   // the next layer's operand is complete
+      }
+      if (!ok) break;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float s = quad_sum(F.head[h][0]), gx = quad_sum(F.head[h][1]), gy = quad_sum(F.head[h][2]), gz = quad_sum(F.gz[h]);
+        if (F.q == 0 && F.valid[h]) {
+          const size_t p = (size_t)F.p[h];
+          a.sdf[p] = s * (1.0f / kTcScaleA) + a.b_last[0];
+          a.grad[3 * p] = gx, a.grad[3 * p + 1] = gy, a.grad[3 * p + 2] = gz;
+        }
+      }
+    } else {
+      for (int l = 0; l < a.n_layers; ++l) {
+        ok = mma_layer(a, P, l, acc);
+        if (!ok) break;
+        const bool head_layer = kColorLike ? (l == a.n_layers - 1) : (l == 7);
+        const bool last_mma = (l == a.n_layers - 1);
+        if (MODE == MLP_BG_SDF && last_mma) epi_layer<MODE, false, false, true, false>(a, F, l, acc);           // the feature rows
+        else if (MODE == MLP_BG_SDF && head_layer) epi_layer<MODE, true, true, false, false>(a, F, l, acc);
+        else if (head_layer) epi_layer<MODE, true, false, false, false>(a, F, l, acc);
+        else if (!kColorLike && l == 3) epi_layer<MODE, false, true, false, true>(a, F, l, acc);
+        else epi_layer<MODE, false, true, false, false>(a, F, l, acc);
+        fence_proxy_async();
+        wg_all(true, P.bar_id);   // the next layer's operand is complete
+      }
+      if (!ok) break;
+      // ---------------------------------------------------------- heads: sum over the 4 threads of each row
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float hs[3];
+#pragma unroll
+        for (int k = 0; k < (kColorLike ? 3 : 1); ++k) hs[k] = quad_sum(F.head[h][k]) * (1.0f / kTcScaleA);  // the head saw activations times kTcScaleA
+        if (F.q == 0 && F.valid[h]) {
+          const size_t p = (size_t)F.p[h];
+          if (kColorLike) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) a.rgb[3 * p + k] = 1.0f / (1.0f + __expf(-(hs[k] + a.b_last[k])));
+          } else {
+            a.sdf[p] = hs[0] + a.b_last[0];
+          }
+        }
+      }
+    }
+    // every thread of the warpgroup has finished with this tile's operand before the next tile's prologue overwrites it
+    wg_all(true, P.bar_id);
   }
 }
 
@@ -1030,7 +906,7 @@ static int tc_init(hold_ctx*) {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_mlp_tc<MLP_COLOR>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<MLP_COLOR>::kSmemBytes);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_mlp_tc<MLP_SDF_REV>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<MLP_SDF_REV>::kSmemBytes);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_mlp_tc<MLP_LINEAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<MLP_LINEAR>::kSmemBytes);
-  if (e != cudaSuccess) { set_error("tcgen05 kernel attribute: %s", cudaGetErrorString(e)); return HOLD_E_CUDA; }
+  if (e != cudaSuccess) { set_error("tensor-core MLP kernel attribute: %s", cudaGetErrorString(e)); return HOLD_E_CUDA; }
   return HOLD_OK;
 }
 
@@ -1105,9 +981,6 @@ static int tc_launch_sdf(hold_ctx* ctx, NodeState& ns, int P, const float* xc, c
   a.passes = (st != nullptr && ctx->sampler_passes >= 1 && ctx->sampler_passes <= 3) ? ctx->sampler_passes : 3;
   a.unscale = kTcUnscale * (1.0f + (float)(ctx->tc_acc_comp >= 0 ? ctx->tc_acc_comp : kTcAccComp) * (1.0f / 16777216.0f));
   const int tiles = ceil_div(P, kTcRows), grid = min(tiles, ctx->sm_count);
-#if defined(HOLD_TC_EXP) && HOLD_TC_EXP == 7
-  if (!rev) { void* rb = nullptr; if (ws_get(ctx, 12, 4096, &rb)) return HOLD_E_CUDA; a.sig = (uint16_t*)rb; }
-#endif
   if (rev) {
     HOLD_REQUIRE(grad != nullptr && feat != nullptr, "sdf eval with gradient needs both grad and feat buffers");
     void* sig = nullptr;

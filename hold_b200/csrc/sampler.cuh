@@ -57,8 +57,8 @@ __device__ __forceinline__ float warp_excl_scan(float v, int lane) {
 // (at::acc_type<float, false>); a CUDA scan accumulates in float.  Either way each prefix is within an ulp of the exact sum.
 // The kernels here keep the TERMS in float (as the reference does) and accumulate the prefixes in double: the inverse-CDF step
 // thresholds cdf[i+1] - cdf[i] at 1e-5 (ray_sampler.py:304), and in empty space that difference is 1e-5 / (1 + 639e-5) =
-// 0.994e-5 — one float ulp of a two-level float scan is enough to flip the branch (measured: 1.8 % of the final samples moved
-// by up to a bin width with float prefixes, tests/test_gpu_sampler_rounds.py).
+// 0.994e-5 — one float ulp of a two-level float scan is enough to flip the branch (with float prefixes a share of the final samples
+// moves by up to a bin width, tests/test_gpu_sampler_rounds.py).
 __device__ __forceinline__ double warp_excl_scan_d(double v, int lane) {
   double x = v;
 #pragma unroll

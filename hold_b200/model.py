@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's call surface for the hot path (SURVEY.md §8b).
 
 Same class names, argument meaning and state_dict keys as the reference (file:line cited per class,
-relative to /root/reference/code/src), so `load_state_dict`, `--load_pose`, `--shape_init` style key
+relative to the reference's code/src), so `load_state_dict`, `--load_pose`, `--shape_init` style key
 filters keep working; every `forward` body is a call into libhold_b200.so.  Inference (eval-mode)
 semantics; the backward kernels are SURVEY §8f rank 2.
 
@@ -413,7 +413,7 @@ class Background(nn.Module):
     def __init__(self, ctx, num_frames, mlp_mode=capi.MLP_FP32):
         super().__init__()
         self.ctx = ctx
-        self.mlp_mode = mlp_mode   # arithmetic of both background nets (HOLD_MLP_FP32 exact fp32, HOLD_MLP_TC tcgen05 split precision)
+        self.mlp_mode = mlp_mode   # arithmetic of both background nets (HOLD_MLP_FP32 exact fp32, HOLD_MLP_TC tensor-core split precision)
         dims = [84] + [256] * 8 + [257]
         self.bg_implicit_network = nn.Module()
         for l in range(9):

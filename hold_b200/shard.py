@@ -25,7 +25,7 @@ def allreduce_flat_(tensors, group=None, average: bool = False):
     gradients per step" of the north star / SURVEY §8e for data-parallel steps (frame-sharded pose refinement,
     optimize_ckpt.py: shared parameters — betas, scene_scale, obj_scale — receive gradient terms from every rank's frames;
     per-frame parameters stay local).  In place; `None` entries are skipped.  Backend-agnostic plumbing
-    (torch.distributed: nccl on the GPU box, gloo in the CPU tests)."""
+    (torch.distributed: nccl on GPUs, gloo in the CPU tests)."""
     import torch
     import torch.distributed as dist
 

@@ -6,8 +6,8 @@ same kinematic tree as MANO: parents of `utils/external/lbs.py:378-383`'s loop)
 and the networks use the reference constructors' init recipe
 (`networks/shape_net.py:51-73`, geometric init).
 
-Everything is generated with numpy's MT19937 / torch's CPU generator so that the
-authoring container and the GPU box produce bit-identical inputs.
+Everything is generated with numpy's MT19937 / torch's CPU generator so that every machine, with or without a GPU,
+produces bit-identical inputs.
 """
 from __future__ import annotations
 

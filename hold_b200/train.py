@@ -2,10 +2,10 @@
 engine/volsdf_utils.py:51-147 with `create_graph=is_training`).
 
 torch.autograd.Functions whose forward AND backward run the algebra of hold_b200/train_algo.py on libhold_b200.so:
-  * every product with a weight matrix: `hold_linear` — the tcgen05 split-precision GEMM (k_mlp_tc<MLP_LINEAR>) against the node's
+  * every product with a weight matrix: `hold_linear` — the tensor-core split-precision GEMM (k_mlp_tc<MLP_LINEAR>) against the node's
     packed weight images (forward and transposed);
   * every pointwise step between them: `hold_train_ew` (hold_b200/csrc/train.cuh);
-  * the weight-gradient reductions dW = D^T A over the points: `hold_wgrad` (k_wgrad_tc: tcgen05 with in-register transposition
+  * the weight-gradient reductions dW = D^T A over the points: `hold_wgrad` (k_wgrad_tc: wgmma with in-register transposition
     of both operands, same split-precision arithmetic);
   * inverse skinning / rigid warp and the pose servers: the existing kernels and their backward twins (hold_inverse_warp_bwd,
     hold_mano_lbs_bwd, hold_object_tf_bwd).
@@ -26,7 +26,7 @@ import torch
 from . import capi, train_algo as T
 from .capi import EwArgs, NodePose, check, lib, ptr, stream_ptr
 
-WGRAD_TC = True   # weight-gradient reductions on hold_wgrad (tcgen05); False: torch.matmul (fp32 library GEMM), kept for A/B timing
+WGRAD_TC = True   # weight-gradient reductions on hold_wgrad (tensor cores); False: torch.matmul (fp32 library GEMM), kept for A/B timing
 
 EW = dict(ACT=0, MUL=1, MULROW=2, U_DZ2=3, DZ=4, EMBED=5, EMBED_VJP=6, EMBED_JVP=7, RELU=8, RELU_BWD=9)
 
@@ -114,7 +114,7 @@ class CudaOps:
         return self._linear(49 + l, A, 256, 256, False)
 
     def wgrad(self, D, A):
-        """D^T A over the points: hold_wgrad (tcgen05, operands rescaled by powers of two) in blocks of <= 256 x 256."""
+        """D^T A over the points: hold_wgrad (tensor cores, operands rescaled by powers of two) in blocks of <= 256 x 256."""
         if not WGRAD_TC:
             return D.T @ A
         P, N = D.shape

@@ -14,7 +14,7 @@ softplus''(z_l) * h_l * q_l added to the pre-activation gradients.  Notation (ro
               dW_l += gbar_l^T u'_{l-1};  second-order seeds  dz2_l = softplus''(z_l) * h_l * q_l  (q_7 := w)
   backward II dA_8 = d_out W_8;  dz_l = dA_{l+1} * s_l + dz2_l;  dW_l += dz_l^T A_l;  dA_l = dz_l W_l;  d_x = E'(x)^T d_e + E''-term
 
-Every product with a weight matrix goes through `ops.lin` / `ops.lin_t` (the tcgen05 split-precision GEMM against the packed
+Every product with a weight matrix goes through `ops.lin` / `ops.lin_t` (the tensor-core split-precision GEMM against the packed
 weight images on the GPU: hold_linear), every weight-gradient reduction over the points through `ops.wgrad` (a plain GEMM), the
 pointwise steps through `ops.*` elementwise kernels.  `TorchOps` (below) runs the same algorithm with torch on the CPU in any
 dtype; tests/test_cpu_train_bwd.py checks it against torch.autograd over the oracle in float64."""

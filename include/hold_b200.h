@@ -1,9 +1,9 @@
-/* hold_b200 — C ABI of the B200-native HOLD volumetric-rendering hot path.
+/* hold_b200 — C ABI of the H100-native HOLD volumetric-rendering hot path.
  *
  * The reference (zc-alexfan/hold) has no FFI/plugin layer: its call surface for this path is a set of
  * Python classes (SURVEY.md §8b).  Each entry point below replaces the body of one of them; the
  * reference-side binding (a ctypes stub inside the unchanged Python class) is shown in INTEGRATION.md.
- * All file:line citations are relative to /root/reference/code/src.
+ * All file:line citations are relative to the reference's code/src.
  *
  * Conventions
  *  - every pointer is a DEVICE pointer to contiguous row-major fp32 unless the name ends in `_host`
@@ -38,7 +38,7 @@ typedef enum hold_status {
 typedef struct hold_ctx hold_ctx;
 
 enum { HOLD_KIND_HAND = 0, HOLD_KIND_OBJECT = 1 };
-/* MLP arithmetic: exact fp32 on CUDA cores, or tcgen05 with fp16 hi/lo split operands, 3 passes (fp32 accumulate). */
+/* MLP arithmetic: exact fp32 on CUDA cores, or wgmma tensor cores with fp16 hi/lo split operands, 3 passes (fp32 accumulate). */
 enum { HOLD_MLP_FP32 = 0, HOLD_MLP_TC = 1 };
 enum { HOLD_MAX_NODES = 4, HOLD_MAX_LAYERS = 9 };
 
@@ -274,7 +274,7 @@ int hold_rgb_eval(hold_ctx* ctx, int node, int B, int P, const float* x_c, const
                   const float* feat, const float* time_code, float* rgb, void* stream);
 
 /* ---- SURVEY §8f rank 2: building blocks of the training backward (hold/hold.py:110-137; algebra in hold_b200/train_algo.py).
- * hold_linear: C[P, nvalid] = A[P, kvalid] . M^T (+ bias) in fp32-level arithmetic (tcgen05, fp16 hi/lo split x 3 passes) against one
+ * hold_linear: C[P, nvalid] = A[P, kvalid] . M^T (+ bias) in fp32-level arithmetic (wgmma, fp16 hi/lo split x 3 passes) against one
  * of the node's packed matrices M, selected by `mat`:
  *    0..8    SDF W_l (networks/shape_net.py:118-126; W_4 carries the skip's 1/sqrt 2, l = 8: the 256 feature rows), bias b_l
  *    16..24  SDF W_l^T (A has N_l columns, C has K_l: 39 for l = 0)
@@ -290,7 +290,7 @@ int hold_linear(hold_ctx* ctx, int node, int mat, int P, const float* A, int lda
                 float* C, int ldc, int nvalid, void* stream);
 
 /* Weight-gradient reduction over the points, out[n, k] = sum_p D[p, n] * A[p, k] (N, K <= 256; out [N, ldo] is overwritten), on
- * tcgen05 with the same fp16 hi/lo split x 3 passes (hold_b200/csrc/wgrad_tc.cuh).  d_scale / a_scale: device scalars (powers of
+ * wgmma with the same fp16 hi/lo split x 3 passes (hold_b200/csrc/wgrad_tc.cuh).  d_scale / a_scale: device scalars (powers of
  * two, NULL = 1) by which D / A are divided before the split; the result is multiplied back. */
 int hold_wgrad(hold_ctx* ctx, int P, const float* D, int ldd, int N, const float* A, int lda, int K, const float* d_scale,
                const float* a_scale, float* out, int ldo, void* stream);

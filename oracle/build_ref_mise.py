@@ -1,19 +1,19 @@
 """Recipe: compile the REFERENCE's own Cython MISE (code/src/libmise/mise.pyx — the only native source in the reference,
-SURVEY §2.2) from where it lies under /root/reference into oracle/_ref/ (git-ignored, never copied into the repo's
-history).  Used only to pin oracle/mise_oracle.py; nothing at test/bench run time on the GPU box needs /root/reference:
-the built module travels with the snapshot.  usage: python oracle/build_ref_mise.py"""
+SURVEY §2.2) from a checkout of the reference named by $HOLD_REFERENCE into oracle/_ref/ (git-ignored, never copied into the
+repo's history).  Used only to pin the MISE restatement (tests/test_cpu_mise.py); nothing at build, test or bench run time
+needs the reference.  usage: python oracle/build_ref_mise.py"""
 import os
 import subprocess
 import sys
 import sysconfig
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = "/root/reference/code/src/libmise/mise.pyx"
+SRC = os.path.join(os.environ.get("HOLD_REFERENCE", ""), "code/src/libmise/mise.pyx")
 OUT = os.path.join(HERE, "_ref")
 
 
 def build():
-    if not os.path.exists(SRC):
+    if not os.environ.get("HOLD_REFERENCE") or not os.path.exists(SRC):
         return None
     os.makedirs(OUT, exist_ok=True)
     ext = sysconfig.get_config_var("EXT_SUFFIX")

@@ -1,12 +1,12 @@
 """CPU ORACLE — TEST INFRASTRUCTURE ONLY.
 
 A plain torch-CPU (fp32) restatement of HOLD's volumetric-rendering hot path, written from the
-reference's behaviour (file:line cited per function, all relative to /root/reference/code/src unless
+reference's behaviour (file:line cited per function, all relative to the reference's code/src unless
 noted).  It exists only to *check* the CUDA path: only `tests/`, `__graft_entry__.smoke()` and
 `bench.py`'s cpu_baseline / `--impl reference` legs may import it.  Nothing under `hold_b200/` does.
 
-Parity status: **pinned against the reference's own modules run in the authoring container**
-(`oracle/ref_harness.py` imports `/root/reference/code/src/{engine,networks,model,...}` behind
+Parity status: **pinned against the reference's own modules**
+(`oracle/ref_harness.py` imports `$HOLD_REFERENCE/code/src/{engine,networks,model,...}` behind
 harness-side shims and compares every function below; the committed fixtures in `tests/golden/` were
 produced by that script).  The reference has no golden vectors / KATs / tests of its own (SURVEY §4),
 and `pytorch3d.ops.knn_points` (pytorch3d 35badc08) is not in the tree, so KNN is restated from its
@@ -393,7 +393,7 @@ def mano_canonical(m, betas):
 
 
 def axis_angle_to_matrix(aa):
-    """/root/reference/common/rot.py:105-138,777-805 (quaternion route)."""
+    """common/rot.py:105-138,777-805 of the reference (quaternion route)."""
     ang = torch.norm(aa, p=2, dim=-1, keepdim=True)
     half = ang * 0.5
     small = ang.abs() < 1e-6

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE (oracle/): signed distance of points to a closed triangle mesh, restating what the reference gets
-from kaolin v0.10.0 (not in /root/reference; parity UNPINNED at that boundary, anchored on the call sites
+from kaolin v0.10.0 (not in the reference's tree; parity UNPINNED at that boundary, anchored on the call sites
 engine/volsdf_utils.py:172-217): `point_to_mesh_distance` = squared distance to the nearest face, `check_sign` =
 inside/outside by ray parity.  Deliberately a different formulation from the kernels' (plane projection + edge
 segments instead of Voronoi regions; ray parity instead of the winding number), in float64."""

@@ -1,6 +1,6 @@
-"""Pin the oracle against the reference's OWN modules (authoring container only).
+"""Pin the oracle against the reference's OWN modules (needs a checkout of the reference, named by $HOLD_REFERENCE).
 
-Imports `/root/reference/code/src/...` unmodified behind harness-side shims (SURVEY §8c):
+Imports `$HOLD_REFERENCE/code/src/...` unmodified behind harness-side shims (SURVEY §8c):
   * `torch.Tensor.cuda` / `nn.Module.cuda` -> identity (the reference hard-codes `.cuda()`, SURVEY D5)
   * stub modules `kaolin`, `trimesh`, `easydict`, `cv2`-free paths, `pytorch3d.ops.knn_points`
     stand-in (squared L2 + topk, the documented contract of pytorch3d 35badc08)
@@ -10,7 +10,8 @@ Usage:
     python oracle/ref_harness.py check      # compare oracle vs reference, print max errors
     python oracle/ref_harness.py golden     # (re)write tests/golden/*.pt from the REFERENCE modules
 
-`/root/reference` does not exist on the GPU box; nothing outside this script reads it.
+Nothing at test or benchmark run time needs the reference checkout; only this script, oracle/build_ref_mise.py and the tests
+that pin the oracle to it (skipped without $HOLD_REFERENCE) read it.
 """
 from __future__ import annotations
 
@@ -23,13 +24,13 @@ import numpy as np
 import torch
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("HOLD_REFERENCE", "")
 sys.path.insert(0, REPO)
 
 
 def install_shims():
     if not os.path.isdir(REF):
-        raise RuntimeError("reference tree not present (this script runs in the authoring container only)")
+        raise RuntimeError("reference tree not present: set $HOLD_REFERENCE to a checkout of the reference")
     torch.Tensor.cuda = lambda self, *a, **k: self
     torch.nn.Module.cuda = lambda self, *a, **k: self
 

@@ -9,8 +9,8 @@ void embed_groups(int D, int deriv, int n_embed, int P, const float* x, const fl
       float v[8];
       const float* q = x + (size_t)p * D;
       unsigned m;
-      if (D == 3) m = deriv ? hold::embed8_inl<3, true>(e0[g], n_embed, q[0], q[1], q[2], 0.f, ew, v) : hold::embed8_inl<3, false>(e0[g], n_embed, q[0], q[1], q[2], 0.f, ew, v);
-      else m = deriv ? hold::embed8_inl<4, true>(e0[g], n_embed, q[0], q[1], q[2], q[3], ew, v) : hold::embed8_inl<4, false>(e0[g], n_embed, q[0], q[1], q[2], q[3], ew, v);
+      if (D == 3) m = deriv ? hold::embedn_inl<3, true>(e0[g], n_embed, q[0], q[1], q[2], 0.f, ew, v) : hold::embedn_inl<3, false>(e0[g], n_embed, q[0], q[1], q[2], 0.f, ew, v);
+      else m = deriv ? hold::embedn_inl<4, true>(e0[g], n_embed, q[0], q[1], q[2], q[3], ew, v) : hold::embedn_inl<4, false>(e0[g], n_embed, q[0], q[1], q[2], q[3], ew, v);
       for (int i = 0; i < 8; ++i) out[((size_t)p * n_groups + g) * 8 + i] = v[i];
       if (p == 0) ok[g] = m;
     }

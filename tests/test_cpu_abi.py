@@ -59,8 +59,8 @@ def test_bad_arguments_are_errors_not_crashes(built):
     assert lib.hold_node_configure(None, 0, None) == -1
 
 
-def test_sass_is_blackwell_native(built):
-    """The shipped .so carries tcgen05 / TMEM / bulk-async SASS for sm_100a (B200_PROFILING.md mnemonics)."""
+def test_sass_is_hopper_native(built):
+    """The shipped .so carries wgmma / bulk-async / mbarrier / setmaxnreg SASS for sm_90a."""
     import subprocess
 
     from hold_b200 import capi
@@ -68,6 +68,6 @@ def test_sass_is_blackwell_native(built):
     out = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
     if not out:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in out
-    for mnem in ("UTCHMMA", "LDTM", "UBLKCP", "UTCBAR"):
+    assert "sm_90a" in out
+    for mnem in ("HGMMA", "UBLKCP", "SYNCS", "USETMAXREG"):
         assert mnem in out, f"{mnem} missing from SASS"

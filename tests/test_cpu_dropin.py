@@ -1,5 +1,5 @@
-"""hold_b200.dropin adaptors carry the reference's own call signatures (SURVEY §8b).  In the authoring container (where
-/root/reference exists) they are compared with `inspect.signature` of the reference's classes, imported behind the harness
+"""hold_b200.dropin adaptors carry the reference's own call signatures (SURVEY §8b).  Where $HOLD_REFERENCE names a checkout
+of the reference they are compared with `inspect.signature` of the reference's classes, imported behind the harness
 shims in a separate interpreter (the shims patch torch.Tensor.cuda); elsewhere only the committed copy of those signatures
 (tests/golden/reference_signatures.json, written by this test when the reference is present) is checked."""
 import inspect
@@ -37,7 +37,7 @@ import sys, json, inspect, importlib
 sys.path.insert(0, %r); sys.path.insert(0, %r)
 from oracle import ref_harness
 ref_harness.install_shims()
-sys.path.insert(0, '/root/reference/code'); sys.path.insert(0, '/root/reference')
+sys.path.insert(0, ref_harness.REF + '/code'); sys.path.insert(0, ref_harness.REF)
 out = {}
 import types
 class _Stub(types.ModuleType):          # third-party packages the reference imports but this container lacks (matplotlib, trimesh, ...)
@@ -87,7 +87,7 @@ def _sig(spec):
 
 
 def _reference_signatures():
-    if os.path.isdir("/root/reference"):
+    if os.path.isdir(os.environ.get("HOLD_REFERENCE", "")):
         r = subprocess.run([sys.executable, "-c", _DUMP % (ROOT, os.path.join(ROOT, "oracle"), list(PAIRS) + list(CTORS))], capture_output=True, text=True,
                            timeout=300, cwd=ROOT)
         assert r.returncode == 0, r.stderr[-3000:]

@@ -1,4 +1,4 @@
-"""CPU-only: the Fourier embedding the tcgen05 chains inline (hold_b200/csrc/embed_phases.h, compiled here with g++) against the
+"""CPU-only: the Fourier embedding the tensor-core chains inline (hold_b200/csrc/embed_phases.h, compiled here with g++) against the
 oracle's embedder (engine/embedders.py:48-51 restated, pinned to the reference): values and derivatives for the 39-element
 canonical-point embedding (with and without BARF weights), the 84-element inverted-sphere embedding of the background and the
 27-element view embedding, at every group offset the kernels use (layer-0 operand: e0 = 0, 8, ...; skip columns: e0 = n0 - 217,

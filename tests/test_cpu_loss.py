@@ -1,6 +1,6 @@
 """hold_b200.train.Loss against the REFERENCE's own hold/loss.py Loss module: tests/golden/loss/*.pt hold synthetic training
-outputs and the loss dict the reference module returned for them (written by `python oracle/ref_harness.py golden_loss` in the
-authoring container).  Covers the schedules (w_sem, w_sparse at steps 0 / 12 000 / beyond the milestone), the eikonal lower bound
+outputs and the loss dict the reference module returned for them (written by `python oracle/ref_harness.py golden_loss` with
+$HOLD_REFERENCE naming a checkout of the reference).  Covers the schedules (w_sem, w_sparse at steps 0 / 12 000 / beyond the milestone), the eikonal lower bound
 (the term is dropped below 8e-4), the clamped MANO canonical term and the segmentation-id remapping."""
 import glob
 import os

@@ -6,6 +6,8 @@ import os
 import pytest
 import torch
 
+import golden_io
+
 GOLD = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "*.pt")))
 
 
@@ -28,7 +30,7 @@ def test_oracle_matches_reference_golden(path):
     from oracle import hold_oracle as O
 
     torch.set_num_threads(min(8, os.cpu_count() or 1))
-    rec = torch.load(path)
+    rec = golden_io.load(path)
     sc = synth.make_scene(**rec["scene_kwargs"])
     for nid in sc.node_ids:
         sc.beta[nid] = torch.tensor(rec["beta"])

@@ -1,7 +1,7 @@
 """SURVEY §8f rank 4: the pose servers under autograd (optimize_ckpt.py's `server.forward_param` + backward).
 hold_mano_lbs_bwd / hold_object_tf_bwd against torch.autograd over the oracle (pinned to the reference's own autograd in
 oracle/ref_harness.py check_pose_grads).  The kernels' phase code is already exercised on the CPU
-(tests/test_cpu_pose_bwd.py); green on hardware since round 1, strict since round 2."""
+(tests/test_cpu_pose_bwd.py)."""
 import pytest
 import torch
 

@@ -42,7 +42,7 @@ def scene():
 
 @pytest.fixture(scope="module", params=["fp32", "tc"])
 def setup(ctx, scene, request):
-    """Every stage test runs in both arithmetic modes of the MLPs: exact fp32 on CUDA cores (HOLD_MLP_FP32) and the tcgen05
+    """Every stage test runs in both arithmetic modes of the MLPs: exact fp32 on CUDA cores (HOLD_MLP_FP32) and the tensor-core
     split-precision path (HOLD_MLP_TC) that bench.py and smoke() use — both are held to the ORACLE at the same tolerance."""
     from hold_b200 import capi, scene_io
 

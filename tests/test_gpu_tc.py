@@ -1,4 +1,4 @@
-"""tcgen05 (bf16 x3 split precision) MLP kernels against the exact-fp32 CUDA-core kernels and the oracle."""
+"""Tensor-core (wgmma, fp16 hi/lo split x3) MLP kernels against the exact-fp32 CUDA-core kernels and the oracle."""
 import pytest
 import torch
 

@@ -1,7 +1,7 @@
 """BASELINE configs[4] in miniature — a joint SDF + LBS backward for pose refinement through the kernels:
 L = sum_p c_p * sdf(x_c(p; pose))  ->  d sdf/d x_c (hold_sdf_eval) -> d/d tfs (hold_inverse_warp_bwd) -> d/d pose, betas, transl,
 scale (hold_mano_lbs_bwd), against torch.autograd over the oracle's whole chain.  The pieces' arithmetic runs on the host
-already (tests/test_cpu_{warp,pose}_bwd.py); green on hardware since round 1 (kept isolated), strict since round 2."""
+already (tests/test_cpu_{warp,pose}_bwd.py); the GPU run is kept isolated."""
 import pytest
 import torch
 

@@ -1,6 +1,6 @@
 """Timings of the SURVEY §8f rank-4 rows against their CPU counterparts on the same box (VERDICT r1 item 10):
  (a) canonical mesh value grid at the reference's resolution (res_init 32, 3 upsampling steps -> 257^3 lattice, utils/meshing.py:10-47):
-     GPU MISE + fused tcgen05 SDF queries (meshing.generate_grid) vs the reference's OWN compiled Cython MISE (oracle/_ref) driven
+     GPU MISE + fused tensor-core SDF queries (meshing.generate_grid) vs the reference's OWN compiled Cython MISE (oracle/_ref) driven
      by the oracle's SDF net on the host cores (what hold.py:139-167 runs on the CPU);
  (b) the pose-refinement server path of optimize_ckpt.py (fitting/model.py:113-117): MANO lbs forward + backward for B frames,
      hold_mano_lbs(+_bwd) vs torch autograd through the oracle's lbs() on the host cores.
@@ -56,7 +56,7 @@ if so is not None:
     same = float((np.sign(ref) == np.sign(grid)).mean())
 print(json.dumps({"row": "8f-4a generate_grid (MISE 32 -> 256, canonical object SDF)", "gpu_s": t_gpu, "cpu_reference_s": t_cpu, "speedup": (t_cpu / t_gpu) if t_cpu else None,
                   "sdf_queries": n_q, "cpu_threads": threads, "inside_outside_agreement": same,
-                  "note": "CPU: the reference's own compiled libmise + oracle SDF net (torch fp32); GPU: hold_mise_* + hold_sdf_eval (tcgen05)"}))
+                  "note": "CPU: the reference's own compiled libmise + oracle SDF net (torch fp32); GPU: hold_mise_* + hold_sdf_eval (tensor cores)"}))
 
 # ---------------------------------------------------------------- (b) pose-refinement server path
 from hold_b200.model import MANOServer

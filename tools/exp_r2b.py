@@ -1,10 +1,9 @@
-"""Round-2 GPU experiments (one process; kept as the provenance of profiles/r02_tc_accumulator_bias.md and r02_variants.md --
-section 3 drove KNN kernel variants that have since been removed from the library):
- 1. tcgen05 SDF chains vs float64: signed / max error of sdf (sampler-round kernel and reverse-mode kernel) and of the gradient,
+"""GPU experiments in one process (section 3 drove KNN kernel variants that have since been removed from the library):
+ 1. tensor-core SDF chains vs float64: signed / max error of sdf (sampler-round kernel and reverse-mode kernel) and of the gradient,
     for accumulator compensation factors 1 + c 2^-24 (is the residual a truncation bias of the tensor core's accumulator?)
  2. kernel times: sampler-round SDF launch, reverse-mode launch
  3. hand KNN / inverse-LBS kernel variants inside hold_sample (A/B/A/B order)
- 4. background nets: exact fp32 vs tcgen05"""
+ 4. background nets: exact fp32 vs tensor cores"""
 import ctypes as C
 import os
 import sys
@@ -27,7 +26,7 @@ def timed(fn, n=3):
     return e0.elapsed_time(e1) / n
 
 # ---------------------------------------------------------------- 1. error vs float64
-print("== 1. tcgen05 SDF chains vs float64 (c = accumulator compensation, scale 1 + c 2^-24)")
+print("== 1. tensor-core SDF chains vs float64 (c = accumulator compensation, scale 1 + c 2^-24)")
 for perturb in (0.0, 0.02, 0.05):
     sc = synth.make_scene(H=8, W=8, S=32, nodes=("right", "object"), seed=4, perturb=perturb)
     net = scene_io.build_net(sc, ctx, capi.MLP_TC)
@@ -103,7 +102,7 @@ print(f"  whole foreground step 256x256: {t:.1f} ms ({256 * 256 / t:.1f} k rays/
 
 # ---------------------------------------------------------------- 4. background
 print("== 4. background nets, 256x256 rays")
-for mm, name in ((capi.MLP_FP32, "fp32 CUDA cores"), (capi.MLP_TC, "tcgen05")):
+for mm, name in ((capi.MLP_FP32, "fp32 CUDA cores"), (capi.MLP_TC, "tensor cores")):
     bg, _, _ = scene_io.build_background(sc2, ctx, mlp_mode=mm)
     w = torch.rand(dirs.shape[0], device=dev)
     res = {}

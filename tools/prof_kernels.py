@@ -1,6 +1,6 @@
 """Fixed launch order for ncu captures: [0] k_mlp_tc<0> sdf-only (2^22 points), [1] k_mlp_tc<3> sdf + gradient + feature
 (2^20 points), then one colour-net launch through hold_shade on a small frame.
-  ncu --set full --clock-control none --import-source on -k regex:k_mlp_tc -s 1 -c 1 -o gpurun_out/x python tools/prof_kernels.py"""
+  ncu --set full --clock-control none --import-source on -k regex:k_mlp_tc -s 1 -c 1 -o prof_out/x python tools/prof_kernels.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
