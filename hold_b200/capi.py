@@ -17,6 +17,10 @@ LIB_PATH = os.path.join(_HERE, "libhold_b200.so")
 MAX_NODES, MAX_LAYERS = 4, 9
 KIND_HAND, KIND_OBJECT = 0, 1
 MLP_FP32, MLP_TC = 0, 1
+# hold_linear matrix ids (include/hold_b200.h), for a node's nets and the background's (node -1) alike: skip net W_l = MAT_SKIP_W + l,
+# W_l^T = MAT_SKIP_WT + l; colour net W_l = MAT_COLOUR_W + l; lin0^T to the features = MAT_COLOUR_WT, to the other inputs =
+# MAT_COLOUR_WT + 1, W_l^T = MAT_COLOUR_WT + 1 + l (l >= 1)
+MAT_SKIP_W, MAT_SKIP_WT, MAT_COLOUR_W, MAT_COLOUR_WT = 0, 16, 32, 48
 
 fp = C.c_void_p  # device pointers travel as void*
 

@@ -31,8 +31,6 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-enum WsSlot { WS_Z = 0, WS_SDF, WS_ZNEW, WS_SDFNEW, WS_BETA, WS_FAR, WS_XC, WS_SSDF, WS_GRAD, WS_FEAT, WS_PE, WS_ZTMP, WS_SIG, WS_BGSDF, WS_BGFEAT, WS_BGRGB, WS_COUNT };
-
 int ws_get(hold_ctx* ctx, int slot, size_t bytes, void** out) {
   Buffer& b = ctx->ws[slot];
   if (b.bytes < bytes) {
@@ -73,24 +71,188 @@ static int check_node(hold_ctx* ctx, int node, bool need_weights) {
   return HOLD_OK;
 }
 
-// ------------------------------------------------------------------------------------------------ MLP launches
-static int fill_sdf_args(const NodeState& ns, SimtArgs& a, bool jvp) {
-  a.n_layers = jvp ? 9 : 8;
-  for (int l = 0; l < a.n_layers; ++l) {
-    a.L[l].Wt = ns.sdf.Wt[l], a.L[l].bias = ns.sdf.bias[l], a.L[l].Kpad = ns.sdf.Kpad[l], a.L[l].N = ns.sdf.N[l];
-  }
-  a.w_last = ns.sdf.w_last, a.b_last = ns.sdf.b_last;
+// ------------------------------------------------------------------------------------------------ the two MLP shapes
+// Skip net (ImplicitNet, networks/shape_net.py:13-49, and the background's implicit net): 9 Softplus layers, lin0 -> 256 x3 ->
+// lin3 (256 - d_skip) -> [a_3 | embedding] / sqrt 2 -> 256 x4 -> lin8 (257: row 0 the sdf head, rows 1..256 the feature vector).
+struct SkipNetShape {
+  const char* name;   // in error messages
+  int in_dim0;        // lin0 inputs of the caller's weights
+  int k_in;           // lin0 inputs packed (the hand's 45 pose columns multiply zeros, shape_net.py:104-106)
+  int d_skip;         // embedding columns re-fed at the skip
+  int tc_kpad0;       // lin0's K padded in the tensor-core image
+  bool weight_norm;   // weight_g allowed
+  int n_out(int l) const { return l == 3 ? kHidden - d_skip : kHidden; }   // packed outputs (lin8: the feature rows)
+  float scale(int l) const { return l == 4 ? (float)(1.0 / sqrt(2.0)) : 1.0f; }   // skip_in: cat([x, input]) / sqrt(2)
+  int row_off(int l) const { return l == 8 ? 1 : 0; }   // lin8 row 0 is the sdf head (packed apart), rows 1..256 the features
+};
+// Colour net (RenderingNet, networks/texture_net.py:13-44, and the background's rendering net): lin0 over k0 inputs, n_hidden
+// ReLU layers of `width` outputs in all, a 3-row sigmoid head.  Its tensor-core lin0 takes the 256 features first in A.
+struct ColourNetShape {
+  const char* name;
+  int k0;             // lin0 inputs
+  int lead;           // lin0 inputs before the features: [x_c, n, pose embed] (| time code after them) / [view PE-4, frame code]
+  int width;          // hidden width
+  int n_hidden;       // GEMM layers before the head
+  bool weight_norm;
+};
+static SkipNetShape node_sdf_shape(bool hand) { return {"SDF", hand ? kEmbed + 45 : kEmbed, kEmbed, kEmbed, 64, true}; }
+static ColourNetShape node_rgb_shape(bool hand) { return {"colour", hand ? 270 : 302, 14, 256, 4, true}; }
+constexpr SkipNetShape kBgSdfShape = {"bg", kBgEmbed + kBgFrame, kBgEmbed + kBgFrame, kBgEmbed, 128, false};
+constexpr ColourNetShape kBgRgbShape = {"bg colour", kBgView + kBgFrame + kFeat, kBgView + kBgFrame, 128, 1, false};
+
+static int check_layer_tensors(const hold_mlp_weights* w, int l, const char* name, bool weight_norm) {
+  HOLD_REQUIRE(w->weight_v[l] && w->bias[l], "%s lin%d has NULL tensors", name, l);
+  HOLD_REQUIRE(weight_norm || !w->weight_g[l], "%s lin%d has weight_g, but this net has no weight-norm", name, l);
   return HOLD_OK;
+}
+
+static int check_skip_net(const hold_mlp_weights* w, const SkipNetShape& s) {
+  HOLD_REQUIRE(w->n_layers == 9, "%s net must have 9 layers, got %d", s.name, w->n_layers);
+  HOLD_REQUIRE(w->in_dim[0] == s.in_dim0, "%s lin0 in_dim %d, expected %d", s.name, w->in_dim[0], s.in_dim0);
+  for (int l = 0; l < 9; ++l) {
+    const int eo = (l == 8) ? kFeat + 1 : s.n_out(l), ei = (l == 0) ? s.in_dim0 : kHidden;
+    HOLD_REQUIRE(w->out_dim[l] == eo && w->in_dim[l] == ei, "%s lin%d is %dx%d, expected %dx%d", s.name, l, w->out_dim[l], w->in_dim[l], eo, ei);
+    int rc = check_layer_tensors(w, l, s.name, s.weight_norm);
+    if (rc) return rc;
+  }
+  return HOLD_OK;
+}
+
+static int check_colour_net(const hold_mlp_weights* w, const ColourNetShape& s) {
+  HOLD_REQUIRE(w->n_layers == s.n_hidden + 1, "%s net must have %d layers, got %d", s.name, s.n_hidden + 1, w->n_layers);
+  HOLD_REQUIRE(w->in_dim[0] == s.k0, "%s lin0 in_dim %d, expected %d", s.name, w->in_dim[0], s.k0);
+  for (int l = 0; l <= s.n_hidden; ++l) {
+    const int eo = (l == s.n_hidden) ? 3 : s.width, ei = (l == 0) ? s.k0 : s.width;
+    HOLD_REQUIRE(w->out_dim[l] == eo && w->in_dim[l] == ei, "%s lin%d is %dx%d, expected %dx%d", s.name, l, w->out_dim[l], w->in_dim[l], eo, ei);
+    int rc = check_layer_tensors(w, l, s.name, s.weight_norm);
+    if (rc) return rc;
+  }
+  return HOLD_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ packing
+// Both packers fold weight-norm and write the fp32 layout and the head; with `tc` also the tensor-core forward and transposed
+// images and the scaled biases.  Buffers are allocated on first use and rewritten in place on every later call.
+static int pack_skip_net(hold_ctx* ctx, PackedNet& m, const hold_mlp_weights* w, const SkipNetShape& s, bool tc, cudaStream_t st) {
+  int rc;
+  m.n_layers = 9;
+  for (int l = 0; l < 9; ++l) {
+    const int K = (l == 0) ? s.k_in : kHidden, Kpad = round_up(K, kKC);
+    m.K[l] = K, m.Kpad[l] = Kpad, m.N[l] = s.n_out(l);
+    if ((rc = dev_alloc(&m.Wt[l], (size_t)Kpad * 256))) return rc;
+    if ((rc = dev_alloc(&m.bias[l], 256))) return rc;
+    k_pack_layer<<<256, 128, 0, st>>>(w->weight_v[l], w->weight_g[l], w->bias[l], w->in_dim[l], s.row_off(l), 0, K, m.N[l], Kpad, s.scale(l),
+                                      m.Wt[l], m.bias[l]);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  if ((rc = dev_alloc(&m.w_last, 256))) return rc;
+  if ((rc = dev_alloc(&m.b_last, 4))) return rc;
+  k_pack_rows<<<1, 128, 0, st>>>(w->weight_v[8], w->weight_g[8], w->bias[8], 256, 0, 1, m.w_last, m.b_last);
+  HOLD_LAUNCH_CHECK(ctx);
+  if (!tc) return HOLD_OK;
+  for (int l = 0; l < 9; ++l) {
+    const int kpad = (l == 0) ? s.tc_kpad0 : 256;
+    m.nst[l] = kpad / 32;
+    if (!m.img[l]) HOLD_CUDA(cudaMalloc((void**)&m.img[l], (size_t)m.nst[l] * kTcStageBytes));
+    k_tc_pack<<<256, 128, 0, st>>>(w->weight_v[l], w->weight_g[l], w->in_dim[l], s.row_off(l), m.N[l], m.K[l], kpad, s.scale(l), 0, m.img[l]);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  for (int l = 0; l < 9; ++l) {  // W_l^T: layers 7..0 for the reverse-mode gradient, all 9 for the training backward
+    if (!m.imgT[l]) HOLD_CUDA(cudaMalloc((void**)&m.imgT[l], (size_t)8 * kTcStageBytes));
+    k_tc_pack_T<<<256, 256, 0, st>>>(w->weight_v[l], w->weight_g[l], w->in_dim[l], s.row_off(l), m.N[l], m.K[l], 0, 0, s.scale(l), m.imgT[l]);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  if (!m.bias_s) HOLD_CUDA(cudaMalloc((void**)&m.bias_s, 9 * 256 * sizeof(float)));
+  for (int l = 0; l < 9; ++l) {  // lin8 (the feature rows) is added unscaled
+    k_scale_vec<<<1, 256, 0, st>>>(m.bias[l], 256, l == 8 ? 1.0f : kTcScaleA, m.bias_s + 256 * l);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  return HOLD_OK;
+}
+
+static int pack_colour_net(hold_ctx* ctx, PackedNet& m, const hold_mlp_weights* w, const ColourNetShape& s, bool tc, cudaStream_t st) {
+  int rc;
+  const int H = s.n_hidden;
+  m.n_layers = H;
+  for (int l = 0; l < H; ++l) {
+    const int K = (l == 0) ? s.k0 : s.width, Kpad = round_up(K, kKC);
+    m.K[l] = K, m.Kpad[l] = Kpad, m.N[l] = s.width;
+    if ((rc = dev_alloc(&m.Wt[l], (size_t)Kpad * 256))) return rc;
+    if ((rc = dev_alloc(&m.bias[l], 256))) return rc;
+    k_pack_layer<<<256, 128, 0, st>>>(w->weight_v[l], w->weight_g[l], w->bias[l], w->in_dim[l], 0, 0, K, s.width, Kpad, 1.0f, m.Wt[l], m.bias[l]);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  if ((rc = dev_alloc(&m.w_last, 3 * s.width))) return rc;
+  if ((rc = dev_alloc(&m.b_last, 4))) return rc;
+  k_pack_rows<<<3, 128, 0, st>>>(w->weight_v[H], w->weight_g[H], w->bias[H], s.width, 0, 3, m.w_last, m.b_last);
+  HOLD_LAUNCH_CHECK(ctx);
+  if (!tc) return HOLD_OK;
+  for (int l = 0; l < H; ++l) {  // lin0: A = [feature (256) | the other inputs], K padded to 320
+    const int kpad = (l == 0) ? 320 : 256;
+    m.nst[l] = kpad / 32;
+    if (!m.img[l]) HOLD_CUDA(cudaMalloc((void**)&m.img[l], (size_t)m.nst[l] * kTcStageBytes));
+    k_tc_pack<<<256, 128, 0, st>>>(w->weight_v[l], w->weight_g[l], w->in_dim[l], 0, s.width, m.K[l], kpad, 1.0f, l == 0 ? s.lead : 0, m.img[l]);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  for (int i = 0; i <= H; ++i) {  // transposes for the training backward: lin0 in two parts (its K = 320 > 256), then lin1..
+    const int l = (i < 2) ? 0 : i - 1;
+    if (!m.imgT[i]) HOLD_CUDA(cudaMalloc((void**)&m.imgT[i], (size_t)8 * kTcStageBytes));
+    k_tc_pack_T<<<256, 256, 0, st>>>(w->weight_v[l], w->weight_g[l], w->in_dim[l], 0, s.width, w->in_dim[l], i == 0 ? 1 : (i == 1 ? 2 : 0), s.lead,
+                                     1.0f, m.imgT[i]);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  if (!m.bias_s) HOLD_CUDA(cudaMalloc((void**)&m.bias_s, (size_t)H * 256 * sizeof(float)));
+  for (int l = 0; l < H; ++l) {
+    k_scale_vec<<<1, 256, 0, st>>>(m.bias[l], 256, kTcScaleA, m.bias_s + 256 * l);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  if (s.width < 256) {  // the tensor-core head reads 256 columns
+    if (!m.w_last_tc) HOLD_CUDA(cudaMalloc((void**)&m.w_last_tc, 3 * 256 * sizeof(float)));
+    k_pad_rows<<<3, 256, 0, st>>>(m.w_last, 3, s.width, 256, m.w_last_tc);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  return HOLD_OK;
+}
+
+static void free_net(PackedNet& m) {
+  for (int l = 0; l < HOLD_MAX_LAYERS; ++l) cudaFree(m.Wt[l]), cudaFree(m.bias[l]), cudaFree(m.img[l]), cudaFree(m.imgT[l]);
+  cudaFree(m.bias_s), cudaFree(m.w_last), cudaFree(m.b_last), cudaFree(m.w_last_tc);
+}
+
+// hold_linear's matrix ids (include/hold_b200.h), the same for a node's nets and the background's
+struct LinearMat {
+  const uint8_t* img = nullptr;
+  const float* bias = nullptr;
+  int nst = 8, kmax = 0, nmax = 0;
+};
+static LinearMat linear_mat(const PackedNet& sdf, const PackedNet& rgb, int mat) {
+  if (mat >= 0 && mat < sdf.n_layers) return {sdf.img[mat], sdf.bias[mat], sdf.nst[mat], sdf.K[mat], sdf.N[mat]};
+  if (mat >= 16 && mat < 16 + sdf.n_layers) { const int l = mat - 16; return {sdf.imgT[l], nullptr, 8, sdf.N[l], sdf.K[l]}; }
+  if (mat >= 32 && mat < 32 + rgb.n_layers) { const int l = mat - 32; return {rgb.img[l], rgb.bias[l], rgb.nst[l], 32 * rgb.nst[l], rgb.N[l]}; }
+  if (mat >= 48 && mat <= 48 + rgb.n_layers) {  // lin0^T to the features / to the other inputs (at most 64), then lin1..^T
+    const int i = mat - 48;
+    return {rgb.imgT[i], nullptr, 8, rgb.N[i < 2 ? 0 : i - 1], i == 0 ? kFeat : (i == 1 ? 64 : rgb.K[i - 1])};
+  }
+  return {};
+}
+
+// ------------------------------------------------------------------------------------------------ MLP launches
+// SimtArgs / BgArgs: layers 0 .. n-1 of a packed net's fp32 chain and its head
+template <class Args>
+static void simt_layers(const PackedNet& m, int n, Args& a) {
+  a.n_layers = n;
+  for (int l = 0; l < n; ++l) a.L[l].Wt = m.Wt[l], a.L[l].bias = m.bias[l], a.L[l].Kpad = m.Kpad[l], a.L[l].N = m.N[l];
+  a.w_last = m.w_last, a.b_last = m.b_last;
 }
 
 static int launch_sdf(hold_ctx* ctx, NodeState& ns, int P, const float* xc, const float* embed_w, float* sdf,
                       float* grad, float* feat, const SamplerState* st, cudaStream_t s) {
   if (P <= 0) return HOLD_OK;
   const bool jvp = (grad != nullptr) || (feat != nullptr);
-  if (ns.cfg.mlp_mode == HOLD_MLP_TC) return tc_launch_sdf(ctx, ns, P, xc, embed_w, sdf, grad, feat, st, s);
+  if (ns.cfg.mlp_mode == HOLD_MLP_TC) return tc_launch_sdf(ctx, ns.sdf, P, xc, embed_w, sdf, grad, feat, st, s);
   SimtArgs a;
   memset(&a, 0, sizeof(a));
-  fill_sdf_args(ns, a, jvp);
+  simt_layers(ns.sdf, jvp ? 9 : 8, a);
   a.P = P, a.xc = xc, a.embed_w = embed_w, a.sdf = sdf, a.grad = grad, a.feat = feat, a.st = st;
   if (jvp) {
     HOLD_REQUIRE(grad != nullptr && feat != nullptr, "sdf eval with gradient needs both grad and feat buffers");
@@ -107,14 +269,10 @@ static int launch_sdf(hold_ctx* ctx, NodeState& ns, int P, const float* xc, cons
 static int launch_rgb(hold_ctx* ctx, NodeState& ns, int P, int pts_per_frame, const float* xc, const float* normal,
                       const float* pe, const float* feat, const float* time_code, float* rgb, cudaStream_t s) {
   if (P <= 0) return HOLD_OK;
-  if (ns.cfg.mlp_mode == HOLD_MLP_TC) return tc_launch_rgb(ctx, ns, P, pts_per_frame, xc, normal, pe, feat, time_code, rgb, s);
+  if (ns.cfg.mlp_mode == HOLD_MLP_TC) return tc_launch_rgb(ctx, ns.rgb, P, pts_per_frame, xc, normal, pe, feat, time_code, rgb, s);
   SimtArgs a;
   memset(&a, 0, sizeof(a));
-  a.n_layers = 4;
-  for (int l = 0; l < 4; ++l) {
-    a.L[l].Wt = ns.rgb.Wt[l], a.L[l].bias = ns.rgb.bias[l], a.L[l].Kpad = ns.rgb.Kpad[l], a.L[l].N = ns.rgb.N[l];
-  }
-  a.w_last = ns.rgb.w_last, a.b_last = ns.rgb.b_last;
+  simt_layers(ns.rgb, ns.rgb.n_layers, a);
   a.P = P, a.xc = xc, a.normal = normal, a.pose_embed = pe, a.feat = const_cast<float*>(feat), a.time_code = time_code;
   a.pts_per_frame = pts_per_frame, a.k0 = ns.rgb.K[0], a.rgb = rgb;
   int tiles = ceil_div(P, kTileRows);
@@ -195,8 +353,6 @@ int hold_ctx_create(hold_ctx** out, int device) {
   const int samp_smem = 4 * 6 * kMaxZ * (int)sizeof(float);
   HOLD_CUDA(cudaFuncSetAttribute(k_sampler_merge_beta, cudaFuncAttributeMaxDynamicSharedMemorySize, samp_smem));
   HOLD_CUDA(cudaFuncSetAttribute(k_sampler_resample, cudaFuncAttributeMaxDynamicSharedMemorySize, samp_smem));
-  const int mano_smem = (2 * kVerts * 3 + kJoints * 3 + kJoints * 9 + 136 + 2 * kJoints * 16 + 16) * (int)sizeof(float);
-  (void)mano_smem;
   HOLD_CUDA(cudaFuncSetAttribute(k_bg_mlp<BG_SDF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBgSmemBytes));
   HOLD_CUDA(cudaFuncSetAttribute(k_bg_mlp<BG_RGB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBgSmemBytes));
   int rc = tc_init(ctx);
@@ -210,36 +366,13 @@ int hold_ctx_create(hold_ctx** out, int device) {
 int hold_ctx_destroy(hold_ctx* ctx) {
   if (!ctx) return HOLD_OK;
   cudaSetDevice(ctx->device);
-  for (int i = 0; i < 24; ++i)
-    if (ctx->ws[i].p) cudaFree(ctx->ws[i].p);
-  for (int n = 0; n < HOLD_MAX_NODES; ++n) {
-    NodeState& ns = ctx->nodes[n];
-    for (int l = 0; l < HOLD_MAX_LAYERS; ++l) {
-      if (ns.sdf.Wt[l]) cudaFree(ns.sdf.Wt[l]);
-      if (ns.sdf.bias[l]) cudaFree(ns.sdf.bias[l]);
-      if (ns.rgb.Wt[l]) cudaFree(ns.rgb.Wt[l]);
-      if (ns.rgb.bias[l]) cudaFree(ns.rgb.bias[l]);
-    }
-    float* ptrs[] = {ns.sdf.w_last, ns.sdf.b_last, ns.rgb.w_last, ns.rgb.b_last, ns.lin_pose_w, ns.lin_pose_b, ns.cano_verts, ns.skin_w};
-    for (float* p : ptrs)
-      if (p) cudaFree(p);
-    if (ns.sstate) cudaFree(ns.sstate);
-    if (ns.knn_perm) cudaFree(ns.knn_perm);
-    tc_free(ns);
+  for (Buffer& b : ctx->ws) cudaFree(b.p);
+  for (NodeState& ns : ctx->nodes) {
+    free_net(ns.sdf), free_net(ns.rgb);
+    cudaFree(ns.lin_pose_w), cudaFree(ns.lin_pose_b), cudaFree(ns.cano_verts), cudaFree(ns.skin_w), cudaFree(ns.sstate), cudaFree(ns.knn_perm);
   }
-  tc_bg_free(ctx->bg_tc);
-  for (int l = 0; l < HOLD_MAX_LAYERS; ++l) {
-    if (ctx->bg_sdf.Wt[l]) cudaFree(ctx->bg_sdf.Wt[l]);
-    if (ctx->bg_sdf.bias[l]) cudaFree(ctx->bg_sdf.bias[l]);
-    if (ctx->bg_rgb.Wt[l]) cudaFree(ctx->bg_rgb.Wt[l]);
-    if (ctx->bg_rgb.bias[l]) cudaFree(ctx->bg_rgb.bias[l]);
-  }
-  {
-    float* ptrs[] = {ctx->bg_sdf.w_last, ctx->bg_sdf.b_last, ctx->bg_rgb.w_last, ctx->bg_rgb.b_last};
-    for (float* p : ptrs)
-      if (p) cudaFree(p);
-  }
-  if (ctx->dev_err) cudaFree(ctx->dev_err);
+  free_net(ctx->bg_sdf), free_net(ctx->bg_rgb);
+  cudaFree(ctx->dev_err);
   delete ctx;
   return HOLD_OK;
 }
@@ -287,66 +420,13 @@ int hold_node_set_weights(hold_ctx* ctx, int node, const hold_mlp_weights* sdf, 
   NodeState& ns = ctx->nodes[node];
   cudaStream_t s = (cudaStream_t)stream;
   const bool hand = ns.cfg.kind == HOLD_KIND_HAND;
-  // ---- SDF net: dims [39(+45)] ->256 x3 -> 217 (+39) ->256 x4 -> 257 (networks/shape_net.py:13-49)
-  HOLD_REQUIRE(sdf->n_layers == 9, "SDF net must have 9 layers, got %d", sdf->n_layers);
-  HOLD_REQUIRE(sdf->in_dim[0] == (hand ? kEmbed + 45 : kEmbed), "SDF lin0 in_dim %d unexpected for this node kind", sdf->in_dim[0]);
-  for (int l = 0; l < 9; ++l) {
-    int eo = (l == 3) ? kHidden - kEmbed : (l == 8 ? kFeat + 1 : kHidden);
-    int ei = (l == 0) ? sdf->in_dim[0] : kHidden;
-    HOLD_REQUIRE(sdf->out_dim[l] == eo && sdf->in_dim[l] == ei, "SDF lin%d is %dx%d, expected %dx%d", l, sdf->out_dim[l], sdf->in_dim[l], eo, ei);
-    HOLD_REQUIRE(sdf->weight_v[l] && sdf->bias[l], "SDF lin%d has NULL tensors", l);
-  }
-  for (int l = 0; l < 9; ++l) {
-    int K = (l == 0) ? kEmbed : kHidden;
-    int Kpad = round_up(K, kKC);
-    int N = (l == 3) ? kHidden - kEmbed : kHidden;
-    int row_off = (l == 8) ? 1 : 0;  // lin8 row 0 is the sdf head, rows 1..256 the feature vector
-    ns.sdf.K[l] = K, ns.sdf.N[l] = N, ns.sdf.Kpad[l] = Kpad, ns.sdf.Npad[l] = 256;
-    rc = dev_alloc(&ns.sdf.Wt[l], (size_t)Kpad * 256);
-    if (rc) return rc;
-    rc = dev_alloc(&ns.sdf.bias[l], 256);
-    if (rc) return rc;
-    float scale = (l == 4) ? (float)(1.0 / sqrt(2.0)) : 1.0f;  // skip_in: cat([x, input]) / sqrt(2)
-    k_pack_layer<<<256, 128, 0, s>>>(sdf->weight_v[l], sdf->weight_g[l], sdf->bias[l], sdf->in_dim[l], row_off, 0, K, N,
-                                     Kpad, scale, ns.sdf.Wt[l], ns.sdf.bias[l]);
-    HOLD_LAUNCH_CHECK(ctx);
-  }
-  ns.sdf.n_layers = 9;
-  rc = dev_alloc(&ns.sdf.w_last, 256);
-  if (rc) return rc;
-  rc = dev_alloc(&ns.sdf.b_last, 4);
-  if (rc) return rc;
-  k_pack_rows<<<1, 128, 0, s>>>(sdf->weight_v[8], sdf->weight_g[8], sdf->bias[8], 256, 0, 1, ns.sdf.w_last, ns.sdf.b_last);
-  HOLD_LAUNCH_CHECK(ctx);
-  // ---- colour net: [270|302] -> 256 x4 -> 3 (networks/texture_net.py:13-44)
-  HOLD_REQUIRE(rgb->n_layers == 5, "colour net must have 5 layers, got %d", rgb->n_layers);
-  const int k0 = hand ? 270 : 302;
-  HOLD_REQUIRE(rgb->in_dim[0] == k0, "colour lin0 in_dim %d, expected %d", rgb->in_dim[0], k0);
-  for (int l = 0; l < 5; ++l) {
-    int eo = (l == 4) ? 3 : 256, ei = (l == 0) ? k0 : 256;
-    HOLD_REQUIRE(rgb->out_dim[l] == eo && rgb->in_dim[l] == ei, "colour lin%d is %dx%d, expected %dx%d", l, rgb->out_dim[l], rgb->in_dim[l], eo, ei);
-    HOLD_REQUIRE(rgb->weight_v[l] && rgb->bias[l], "colour lin%d has NULL tensors", l);
-  }
-  for (int l = 0; l < 4; ++l) {
-    int K = (l == 0) ? k0 : 256, Kpad = round_up(K, kKC);
-    ns.rgb.K[l] = K, ns.rgb.N[l] = 256, ns.rgb.Kpad[l] = Kpad, ns.rgb.Npad[l] = 256;
-    rc = dev_alloc(&ns.rgb.Wt[l], (size_t)Kpad * 256);
-    if (rc) return rc;
-    rc = dev_alloc(&ns.rgb.bias[l], 256);
-    if (rc) return rc;
-    k_pack_layer<<<256, 128, 0, s>>>(rgb->weight_v[l], rgb->weight_g[l], rgb->bias[l], rgb->in_dim[l], 0, 0, K, 256, Kpad,
-                                     1.0f, ns.rgb.Wt[l], ns.rgb.bias[l]);
-    HOLD_LAUNCH_CHECK(ctx);
-  }
-  ns.rgb.n_layers = 5;
-  rc = dev_alloc(&ns.rgb.w_last, 3 * 256);
-  if (rc) return rc;
-  rc = dev_alloc(&ns.rgb.b_last, 4);
-  if (rc) return rc;
-  k_pack_rows<<<3, 128, 0, s>>>(rgb->weight_v[4], rgb->weight_g[4], rgb->bias[4], 256, 0, 3, ns.rgb.w_last, ns.rgb.b_last);
-  HOLD_LAUNCH_CHECK(ctx);
+  const SkipNetShape ss = node_sdf_shape(hand);
+  const ColourNetShape cs = node_rgb_shape(hand);
+  if ((rc = check_skip_net(sdf, ss)) || (rc = check_colour_net(rgb, cs))) return rc;
+  HOLD_REQUIRE(!hand || (lin_pose_w && lin_pose_b), "hand node needs lin_pose weights");
+  // both arithmetic modes are packed: hold_linear (the training backward) uses the tensor-core images in either mode
+  if ((rc = pack_skip_net(ctx, ns.sdf, sdf, ss, true, s)) || (rc = pack_colour_net(ctx, ns.rgb, rgb, cs, true, s))) return rc;
   if (hand) {
-    HOLD_REQUIRE(lin_pose_w && lin_pose_b, "hand node needs lin_pose weights");
     rc = dev_alloc(&ns.lin_pose_w, 8 * 45);
     if (rc) return rc;
     rc = dev_alloc(&ns.lin_pose_b, 8);
@@ -354,8 +434,6 @@ int hold_node_set_weights(hold_ctx* ctx, int node, const hold_mlp_weights* sdf, 
     HOLD_CUDA(cudaMemcpyAsync(ns.lin_pose_w, lin_pose_w, 8 * 45 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     HOLD_CUDA(cudaMemcpyAsync(ns.lin_pose_b, lin_pose_b, 8 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   }
-  rc = tc_pack(ctx, ns, sdf, rgb, s);
-  if (rc) return rc;
   ns.has_weights = true;
   return HOLD_OK;
 }
@@ -827,7 +905,7 @@ int hold_inverse_warp_bwd(hold_ctx* ctx, int node, int B, int P, const float* x,
   cudaStream_t s = (cudaStream_t)stream;
   const int nb = max(1, ceil_div(P, 128));
   void* part = nullptr;
-  if ((rc = ws_get(ctx, 22 /* WS_WARPBWD */, (size_t)B * nb * warpbwd::kJ * warpbwd::kG * sizeof(float), &part))) return rc;
+  if ((rc = ws_get(ctx, WS_WARPBWD,(size_t)B * nb * warpbwd::kJ * warpbwd::kG * sizeof(float), &part))) return rc;
   dim3 grid(nb, B);
   if (hand) {
     HOLD_REQUIRE(ns.has_rig, "hand node has no rig (hold_node_set_rig)");
@@ -981,7 +1059,7 @@ int hold_debug_set(hold_ctx* ctx, int key, int value) {
 
 /* debug/test hook (not in the public header): workspace slot pointers of the last call */
 int hold_debug_ws_copy(hold_ctx* ctx, int slot, void* dst, size_t bytes) {
-  if (!ctx || slot < 0 || slot >= 24 || ctx->ws[slot].bytes < bytes) return HOLD_E_BADARG;
+  if (!ctx || slot < 0 || slot >= WS_COUNT || ctx->ws[slot].bytes < bytes) return HOLD_E_BADARG;
   HOLD_CUDA(cudaDeviceSynchronize());
   HOLD_CUDA(cudaMemcpy(dst, ctx->ws[slot].p, bytes, cudaMemcpyDeviceToDevice));
   return HOLD_OK;
@@ -991,44 +1069,13 @@ int hold_bg_set_weights(hold_ctx* ctx, const hold_mlp_weights* sdf, const hold_m
   HOLD_REQUIRE(ctx && sdf && rgb, "NULL argument");
   HOLD_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t s = (cudaStream_t)stream;
-  HOLD_REQUIRE(sdf->n_layers == 9 && rgb->n_layers == 2, "background nets: 9 + 2 layers expected");
-  HOLD_REQUIRE(sdf->in_dim[0] == kBgEmbed + kBgFrame, "bg lin0 in_dim %d, expected 116", sdf->in_dim[0]);
-  HOLD_REQUIRE(rgb->in_dim[0] == kBgView + kBgFrame + kFeat && rgb->out_dim[0] == 128 && rgb->out_dim[1] == 3 && rgb->in_dim[1] == 128,
-               "bg colour head must be 315 -> 128 -> 3");
-  PackedMlp& m = ctx->bg_sdf;
-  int rc;
-  for (int l = 0; l < 9; ++l) {
-    const int eo = (l == 3) ? kHidden - kBgEmbed : (l == 8 ? kFeat + 1 : kHidden), ei = (l == 0) ? kBgEmbed + kBgFrame : kHidden;
-    HOLD_REQUIRE(sdf->out_dim[l] == eo && sdf->in_dim[l] == ei, "bg lin%d is %dx%d, expected %dx%d", l, sdf->out_dim[l], sdf->in_dim[l], eo, ei);
-    HOLD_REQUIRE(sdf->weight_v[l] && sdf->bias[l], "bg lin%d has NULL tensors", l);
-    const int K = ei, Kpad = round_up(K, kKC), N = (l == 3) ? kHidden - kBgEmbed : kHidden, row_off = (l == 8) ? 1 : 0;
-    m.K[l] = K, m.N[l] = N, m.Kpad[l] = Kpad, m.Npad[l] = 256;
-    if ((rc = dev_alloc(&m.Wt[l], (size_t)Kpad * 256))) return rc;
-    if ((rc = dev_alloc(&m.bias[l], 256))) return rc;
-    const float scale = (l == 4) ? (float)(1.0 / sqrt(2.0)) : 1.0f;
-    k_pack_layer<<<256, 128, 0, s>>>(sdf->weight_v[l], sdf->weight_g[l], sdf->bias[l], sdf->in_dim[l], row_off, 0, K, N, Kpad, scale, m.Wt[l], m.bias[l]);
-    HOLD_LAUNCH_CHECK(ctx);
-  }
-  m.n_layers = 9;
-  if ((rc = dev_alloc(&m.w_last, 256))) return rc;
-  if ((rc = dev_alloc(&m.b_last, 4))) return rc;
-  k_pack_rows<<<1, 128, 0, s>>>(sdf->weight_v[8], sdf->weight_g[8], sdf->bias[8], 256, 0, 1, m.w_last, m.b_last);
-  HOLD_LAUNCH_CHECK(ctx);
-  PackedMlp& c = ctx->bg_rgb;
-  const int K0 = kBgView + kBgFrame + kFeat, K0pad = round_up(K0, kKC);
-  c.K[0] = K0, c.N[0] = 128, c.Kpad[0] = K0pad, c.Npad[0] = 256;
-  if ((rc = dev_alloc(&c.Wt[0], (size_t)K0pad * 256))) return rc;
-  if ((rc = dev_alloc(&c.bias[0], 256))) return rc;
-  k_pack_layer<<<256, 128, 0, s>>>(rgb->weight_v[0], rgb->weight_g[0], rgb->bias[0], K0, 0, 0, K0, 128, K0pad, 1.0f, c.Wt[0], c.bias[0]);
-  HOLD_LAUNCH_CHECK(ctx);
-  c.n_layers = 2;
-  if ((rc = dev_alloc(&c.w_last, 3 * 128))) return rc;
-  if ((rc = dev_alloc(&c.b_last, 4))) return rc;
-  k_pack_rows<<<3, 128, 0, s>>>(rgb->weight_v[1], rgb->weight_g[1], rgb->bias[1], 128, 0, 3, c.w_last, c.b_last);
-  HOLD_LAUNCH_CHECK(ctx);
   HOLD_REQUIRE(mlp_mode == HOLD_MLP_FP32 || mlp_mode == HOLD_MLP_TC, "bad mlp_mode");
+  int rc;
+  if ((rc = check_skip_net(sdf, kBgSdfShape)) || (rc = check_colour_net(rgb, kBgRgbShape))) return rc;
+  const bool tc = mlp_mode == HOLD_MLP_TC;
+  ctx->has_bg = false;   // until both nets are packed for this mode
+  if ((rc = pack_skip_net(ctx, ctx->bg_sdf, sdf, kBgSdfShape, tc, s)) || (rc = pack_colour_net(ctx, ctx->bg_rgb, rgb, kBgRgbShape, tc, s))) return rc;
   ctx->bg_mlp_mode = mlp_mode;
-  if (mlp_mode == HOLD_MLP_TC && (rc = tc_bg_pack(ctx, ctx->bg_tc, sdf, rgb, s))) return rc;
   ctx->has_bg = true;
   return HOLD_OK;
 }
@@ -1062,20 +1109,18 @@ int hold_background(hold_ctx* ctx, int R, int B, const float* cam_loc, const flo
       for (int n = 0; n < HOLD_MAX_NODES; ++n)
         if (ctx->nodes[n].configured) { a.r_sphere = ctx->nodes[n].cfg.bounding_sphere; break; }
       HOLD_REQUIRE(a.r_sphere > 0.f, "configure a node first (scene_bounding_sphere)");
-      a.n_layers = 9;
-      for (int l = 0; l < 9; ++l) { a.L[l].Wt = ctx->bg_sdf.Wt[l], a.L[l].bias = ctx->bg_sdf.bias[l], a.L[l].Kpad = ctx->bg_sdf.Kpad[l], a.L[l].N = ctx->bg_sdf.N[l]; }
-      a.w_last = ctx->bg_sdf.w_last, a.b_last = ctx->bg_sdf.b_last, a.sdf = sdf_ws, a.feat = feat_ws;
-      if (ctx->bg_mlp_mode == HOLD_MLP_TC && ctx->bg_tc != nullptr) {
-        int rc = tc_bg_launch(ctx, *ctx->bg_tc, P, a.cam, a.dirs, a.frame_code, a.r_sphere, sdf_ws, feat_ws, rgb_ws, s);
+      simt_layers(ctx->bg_sdf, ctx->bg_sdf.n_layers, a);
+      a.sdf = sdf_ws, a.feat = feat_ws;
+      if (ctx->bg_mlp_mode == HOLD_MLP_TC) {
+        int rc = tc_bg_launch(ctx, P, a.cam, a.dirs, a.frame_code, a.r_sphere, sdf_ws, feat_ws, rgb_ws, s);
         if (rc) return rc;
       } else {
         const int tiles = ceil_div(P, kTileRows);
         k_bg_mlp<BG_SDF><<<min(tiles, ctx->sm_count), 256, kBgSmemBytes, s>>>(a);
         HOLD_LAUNCH_CHECK(ctx);
         BgArgs c = a;
-        c.n_layers = 1;
-        c.L[0].Wt = ctx->bg_rgb.Wt[0], c.L[0].bias = ctx->bg_rgb.bias[0], c.L[0].Kpad = ctx->bg_rgb.Kpad[0], c.L[0].N = 128;
-        c.w_last = ctx->bg_rgb.w_last, c.b_last = ctx->bg_rgb.b_last, c.rgb = rgb_ws;
+        simt_layers(ctx->bg_rgb, ctx->bg_rgb.n_layers, c);
+        c.rgb = rgb_ws;
         k_bg_mlp<BG_RGB><<<min(tiles, ctx->sm_count), 256, kBgSmemBytes, s>>>(c);
         HOLD_LAUNCH_CHECK(ctx);
       }
@@ -1105,32 +1150,25 @@ int hold_linear(hold_ctx* ctx, int node, int mat, int P, const float* A, int lda
   HOLD_REQUIRE(P >= 0, "negative P");
   if (P == 0) return HOLD_OK;
   HOLD_REQUIRE(A && C, "NULL argument");
-  const uint8_t* img = nullptr;
-  const float* bias = nullptr;
-  int nst = 8, kmax = 256, nmax = 256;
+  LinearMat m;
   if (node == -1) {   // the background nets (hold_bg_set_weights with HOLD_MLP_TC)
     HOLD_CUDA(cudaSetDevice(ctx->device));
-    HOLD_REQUIRE(ctx->has_bg && ctx->bg_tc != nullptr, "hold_linear(node -1) needs tensor-core background weights (hold_bg_set_weights, HOLD_MLP_TC)");
-    const TcBg& t = *ctx->bg_tc;
-    constexpr int kIn = kBgEmbed + kBgFrame;   // lin0: 116 inputs; the skip at layer 4 re-feeds the 84 embedding columns (lin3: 172 outputs)
-    if (mat >= 0 && mat <= 8) { img = t.sdf_img[mat]; bias = ctx->bg_sdf.bias[mat]; nst = t.sdf_nst[mat]; kmax = (mat == 0) ? kIn : 256; nmax = (mat == 3) ? 256 - kBgEmbed : 256; }
-    else if (mat >= 16 && mat <= 24) { img = t.sdf_imgT[mat - 16]; kmax = (mat == 19) ? 256 - kBgEmbed : 256; nmax = (mat == 16) ? kIn : 256; }
-    else if (mat == 32) { img = t.rgb_img; bias = ctx->bg_rgb.bias[0]; nst = 10; kmax = 320; nmax = 128; }
-    else if (mat == 48 || mat == 49) { img = t.rgb_imgT[mat - 48]; kmax = 128; nmax = (mat == 49) ? 64 : 256; }
+    HOLD_REQUIRE(ctx->has_bg, "hold_linear(node -1) needs tensor-core background weights (hold_bg_set_weights, HOLD_MLP_TC)");
+    if (ctx->bg_mlp_mode != HOLD_MLP_TC) {
+      set_error("hold_linear(node -1): the background weights were last set with HOLD_MLP_FP32; its tensor-core images are not current");
+      return HOLD_E_STATE;
+    }
+    m = linear_mat(ctx->bg_sdf, ctx->bg_rgb, mat);
   } else {
     int rc = check_node(ctx, node, true);
     if (rc) return rc;
-    NodeState& ns = ctx->nodes[node];
-    HOLD_REQUIRE(ns.tc != nullptr, "hold_linear needs the packed tensor-core weight images (hold_node_set_weights)");
-    if (mat >= 0 && mat <= 8) { img = ns.tc->sdf_img[mat]; bias = ns.sdf.bias[mat]; nst = ns.tc->sdf_nst[mat]; kmax = (mat == 0) ? kEmbed : 256; nmax = ns.sdf.N[mat]; }
-    else if (mat >= 16 && mat <= 24) { img = ns.tc->sdf_imgT[mat - 16]; kmax = (mat - 16 == 3) ? kHidden - kEmbed : 256; nmax = (mat == 16) ? kEmbed : 256; }
-    else if (mat >= 32 && mat <= 35) { img = ns.tc->rgb_img[mat - 32]; bias = ns.rgb.bias[mat - 32]; nst = ns.tc->rgb_nst[mat - 32]; kmax = (mat == 32) ? 320 : 256; }
-    else if (mat >= 48 && mat <= 52) { img = ns.tc->rgb_imgT[mat - 48]; nmax = (mat == 49) ? 64 : 256; }
+    m = linear_mat(ctx->nodes[node].sdf, ctx->nodes[node].rgb, mat);
   }
-  HOLD_REQUIRE(img != nullptr, "hold_linear: unknown matrix id %d for node %d", mat, node);
-  HOLD_REQUIRE(kvalid >= 1 && kvalid <= kmax && nvalid >= 1 && nvalid <= nmax, "hold_linear(%d): kvalid %d (max %d) / nvalid %d (max %d)", mat, kvalid, kmax, nvalid, nmax);
-  HOLD_REQUIRE(!add_bias || bias != nullptr, "hold_linear(%d): this matrix has no bias", mat);
-  return tc_launch_linear_img(ctx, img, add_bias ? bias : nullptr, nst, P, A, lda, kvalid, in_scale, C, ldc, nvalid, (cudaStream_t)stream);
+  HOLD_REQUIRE(m.img != nullptr, "hold_linear: unknown matrix id %d for node %d", mat, node);
+  HOLD_REQUIRE(kvalid >= 1 && kvalid <= m.kmax && nvalid >= 1 && nvalid <= m.nmax, "hold_linear(%d): kvalid %d (max %d) / nvalid %d (max %d)", mat, kvalid,
+               m.kmax, nvalid, m.nmax);
+  HOLD_REQUIRE(!add_bias || m.bias != nullptr, "hold_linear(%d): this matrix has no bias", mat);
+  return tc_launch_linear_img(ctx, m.img, add_bias ? m.bias : nullptr, m.nst, P, A, lda, kvalid, in_scale, C, ldc, nvalid, (cudaStream_t)stream);
 }
 
 int hold_wgrad(hold_ctx* ctx, int P, const float* D, int ldd, int N, const float* A, int lda, int K, const float* d_scale,
@@ -1156,7 +1194,7 @@ int hold_pow2_scale(hold_ctx* ctx, int P, int ncols, const float* x, int ld, flo
   HOLD_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t s = (cudaStream_t)stream;
   void* w = nullptr;
-  int rc = ws_get(ctx, 21 /* WS_AMAX */, 256, &w);
+  int rc = ws_get(ctx, WS_AMAX, 256, &w);
   if (rc) return rc;
   // one word per call, rotating through the workspace so that back-to-back calls on a stream never share a counter in flight
   unsigned int* bits = (unsigned int*)w + (ctx->launches & 31);

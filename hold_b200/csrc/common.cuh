@@ -19,8 +19,6 @@ constexpr int kEmbed = 39;     // 3 + 3*2*6 (engine/embedders.py:21-41, multires
 constexpr int kFeat = 256;     // feature_vector_size
 constexpr int kHidden = 256;
 constexpr int kMaxZ = 640;     // n_samples_eval * max_total_iters upper bound supported by the sampler kernels
-constexpr int kSdfLayers = 9;
-constexpr int kRgbLayers = 5;
 
 // device error word bits
 constexpr int kErrRayMiss = 1;
@@ -32,23 +30,31 @@ struct SamplerState {  // device-resident, one per node; written only by single-
   unsigned beta_max_bits[8];  // per round: max over rays of beta (float bits, positive => monotone)
 };
 
-struct PackedMlp {           // fp32 CUDA-core layout: Wt[l] is [Kpad][Npad] (k-major rows, n contiguous)
+// One MLP (node or background, skip net or colour net) packed for both arithmetic modes by pack_skip_net / pack_colour_net
+// (api.cu).  Layers 0 .. n_layers-1 are the GEMM layers; the 1- or 3-row output head is kept apart as plain rows.
+struct PackedNet {
   int n_layers = 0;
-  int K[HOLD_MAX_LAYERS], N[HOLD_MAX_LAYERS], Kpad[HOLD_MAX_LAYERS], Npad[HOLD_MAX_LAYERS];
-  float* Wt[HOLD_MAX_LAYERS] = {nullptr};
-  float* bias[HOLD_MAX_LAYERS] = {nullptr};
-  float* w_last = nullptr;   // SDF: row 0 of the last layer (the sdf output) [256]; RGB: last layer [3][256]
+  int K[HOLD_MAX_LAYERS], Kpad[HOLD_MAX_LAYERS], N[HOLD_MAX_LAYERS];   // packed inputs, K padded to kKC, valid outputs
+  float* Wt[HOLD_MAX_LAYERS] = {nullptr};       // fp32 CUDA-core layout [Kpad][256] (k-major rows, n contiguous)
+  float* bias[HOLD_MAX_LAYERS] = {nullptr};     // [256], zero beyond N
+  uint8_t* img[HOLD_MAX_LAYERS] = {nullptr};    // tensor-core forward images: nst[l] stages of 32 k (mlp_tc.cuh)
+  int nst[HOLD_MAX_LAYERS] = {0};
+  uint8_t* imgT[HOLD_MAX_LAYERS] = {nullptr};   // transposed images, 8 stages each: skip net W_l^T; colour net lin0^T to the
+                                                // features, lin0^T to the other inputs, then W_1..^T
+  float* bias_s = nullptr;                      // [n_layers][256]: the biases as the tensor-core epilogues add them
+  float* w_last = nullptr;                      // head: skip net row 0 of lin8 [256]; colour net [3][hidden width]
   float* b_last = nullptr;
+  float* w_last_tc = nullptr;                   // colour head padded to [3][256] when the hidden width is narrower (tensor cores)
 };
 
-struct TcMlp;  // tensor-core packing, mlp_tc.cuh
-struct TcBg;   // tensor-core packing of the background nets, background_tc.cuh
+// grow-only workspaces of a hold_ctx, one per purpose
+enum WsSlot { WS_Z = 0, WS_SDF, WS_ZNEW, WS_SDFNEW, WS_BETA, WS_FAR, WS_XC, WS_SSDF, WS_GRAD, WS_FEAT, WS_PE, WS_ZTMP, WS_SIG,
+              WS_BGSDF, WS_BGFEAT, WS_BGRGB, WS_AMAX, WS_WARPBWD, WS_COUNT };
 
 struct NodeState {
   bool configured = false, has_weights = false, has_rig = false;
   hold_node_cfg cfg;
-  PackedMlp sdf, rgb;
-  TcMlp* tc = nullptr;
+  PackedNet sdf, rgb;
   float* lin_pose_w = nullptr;  // [8,45]
   float* lin_pose_b = nullptr;  // [8]
   float* cano_verts = nullptr;  // [778,3]
@@ -70,11 +76,10 @@ struct hold_ctx {
   hold::NodeState nodes[HOLD_MAX_NODES];
   int* dev_err = nullptr;
   int64_t launches = 0;
-  hold::Buffer ws[24];  // grow-only workspaces, indexed by purpose (api.cu)
-  hold::PackedMlp bg_sdf, bg_rgb;  // background nets (fp32 CUDA-core layout)
+  hold::Buffer ws[hold::WS_COUNT];
+  hold::PackedNet bg_sdf, bg_rgb;  // background nets (tensor-core images only when bg_mlp_mode is HOLD_MLP_TC)
   bool has_bg = false;
   int bg_mlp_mode = 0;             // HOLD_MLP_* of the background nets (hold_bg_set_weights)
-  hold::TcBg* bg_tc = nullptr;
   int sampler_passes = 3;          // measurement hook (hold_debug_set key 3): MMA passes of the sampler-round SDF launches
   int tc_acc_comp = -1;            // measurement hook (hold_debug_set key 2): accumulator scale 1 + c * 2^-24 in the SDF chains; < 0: kTcAccComp
 };

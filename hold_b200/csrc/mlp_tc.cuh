@@ -56,15 +56,6 @@ __global__ void k_scale_vec(const float* __restrict__ src, int n, float c, float
   if (i < n) dst[i] = c * src[i];
 }
 
-struct TcMlp {
-  uint8_t* sdf_img[HOLD_MAX_LAYERS] = {nullptr};
-  uint8_t* rgb_img[HOLD_MAX_LAYERS] = {nullptr};
-  uint8_t* sdf_imgT[HOLD_MAX_LAYERS] = {nullptr};  // W_l^T images of layers 0..7 for the reverse-mode gradient, 8: feature rows (training)
-  uint8_t* rgb_imgT[6] = {nullptr};                // training backward: [0] W_0^T feature part, [1] W_0^T other inputs, [2..4] W_1..3^T
-  int sdf_nst[HOLD_MAX_LAYERS], rgb_nst[HOLD_MAX_LAYERS];
-  float* bias_s = nullptr;   // [13][256]: biases as the epilogues add them: SDF lin0..7 times kTcScaleA, lin8 (feature rows) plain, colour lin0..3 times kTcScaleA
-};
-
 struct TcArgs {
   int P, n_layers;
   TcLayer L[kTcMaxSteps];
@@ -389,7 +380,7 @@ __device__ __forceinline__ void frag_store_a(const Frag& F, int h, int j, float 
 //   WRITE: the activations are the next MMA's operand (false on the chain's last MMA layer)
 //   FEAT : the layer's outputs are the 256-d feature vector (no activation, stored to global memory)
 //   SKIP : output columns >= a.L[l].N are the point's embedding (the skip connection into the next layer, shape_net.py:116-119)
-// One specialised body per layer kind.  a.L[l].bias is pre-multiplied by kTcScaleA unless FEAT (TcMlp::bias_s).
+// One specialised body per layer kind.  a.L[l].bias is pre-multiplied by kTcScaleA unless FEAT (PackedNet::bias_s).
 template <int MODE, bool HEAD, bool WRITE, bool FEAT, bool SKIP>
 __device__ __forceinline__ void epi_layer(const TcArgs& a, Frag& F, const int l, const float (&acc)[128]) {
   constexpr bool kColorLike = (MODE == MLP_COLOR || MODE == MLP_BG_RGB);
@@ -910,73 +901,23 @@ static int tc_init(hold_ctx*) {
   return HOLD_OK;
 }
 
-static void tc_free(NodeState& ns) {
-  if (!ns.tc) return;
-  for (int l = 0; l < HOLD_MAX_LAYERS; ++l) {
-    if (ns.tc->sdf_img[l]) cudaFree(ns.tc->sdf_img[l]);
-    if (ns.tc->rgb_img[l]) cudaFree(ns.tc->rgb_img[l]);
-    if (ns.tc->sdf_imgT[l]) cudaFree(ns.tc->sdf_imgT[l]);
-    if (l < 6 && ns.tc->rgb_imgT[l]) cudaFree(ns.tc->rgb_imgT[l]);
-  }
-  if (ns.tc->bias_s) cudaFree(ns.tc->bias_s);
-  delete ns.tc;
-  ns.tc = nullptr;
-}
-
-static int tc_pack(hold_ctx* ctx, NodeState& ns, const hold_mlp_weights* sdf, const hold_mlp_weights* rgb, cudaStream_t s) {
-  if (!ns.tc) ns.tc = new TcMlp();
-  TcMlp& t = *ns.tc;
-  for (int l = 0; l < 9; ++l) {
-    const int K = (l == 0) ? kEmbed : kHidden, kpad = (l == 0) ? 64 : 256;
-    const int N = (l == 3) ? kHidden - kEmbed : kHidden;
-    const int row_off = (l == 8) ? 1 : 0;
-    t.sdf_nst[l] = kpad / 32;
-    if (!t.sdf_img[l]) HOLD_CUDA(cudaMalloc((void**)&t.sdf_img[l], (size_t)t.sdf_nst[l] * kTcStageBytes));
-    const float scale = (l == 4) ? (float)(1.0 / sqrt(2.0)) : 1.0f;
-    k_tc_pack<<<256, 128, 0, s>>>(sdf->weight_v[l], sdf->weight_g[l], sdf->in_dim[l], row_off, N, K, kpad, scale, 0, t.sdf_img[l]);
-    HOLD_LAUNCH_CHECK(ctx);
-  }
-  for (int l = 0; l < 9; ++l) {  // W_l^T for the reverse-mode gradient (layers 7..0); l = 8: the feature rows (training backward)
-    const int K_in = (l == 0) ? kEmbed : kHidden, N_out = (l == 3) ? kHidden - kEmbed : kHidden;
-    if (!t.sdf_imgT[l]) HOLD_CUDA(cudaMalloc((void**)&t.sdf_imgT[l], (size_t)8 * kTcStageBytes));
-    const float scale = (l == 4) ? (float)(1.0 / sqrt(2.0)) : 1.0f;
-    k_tc_pack_T<<<256, 256, 0, s>>>(sdf->weight_v[l], sdf->weight_g[l], sdf->in_dim[l], l == 8 ? 1 : 0, N_out, K_in, 0, 0, scale, t.sdf_imgT[l]);
-    HOLD_LAUNCH_CHECK(ctx);
-  }
-  for (int i = 0; i < 5; ++i) {  // colour net transposes for the training backward: lin0 in two parts (its K = 320 > 256), lin1..3
-    const int l = (i < 2) ? 0 : i - 1;
-    if (!t.rgb_imgT[i]) HOLD_CUDA(cudaMalloc((void**)&t.rgb_imgT[i], (size_t)8 * kTcStageBytes));
-    k_tc_pack_T<<<256, 256, 0, s>>>(rgb->weight_v[l], rgb->weight_g[l], rgb->in_dim[l], 0, 256, rgb->in_dim[l], i == 0 ? 1 : (i == 1 ? 2 : 0), 14, 1.0f,
-                                    t.rgb_imgT[i]);
-    HOLD_LAUNCH_CHECK(ctx);
-  }
-  if (!t.bias_s) HOLD_CUDA(cudaMalloc((void**)&t.bias_s, 13 * 256 * sizeof(float)));
-  for (int l = 0; l < 13; ++l) {   // (the fp32 packing of this call has already written ns.sdf.bias / ns.rgb.bias on this stream)
-    k_scale_vec<<<1, 256, 0, s>>>(l < 9 ? ns.sdf.bias[l] : ns.rgb.bias[l - 9], 256, l == 8 ? 1.0f : kTcScaleA, t.bias_s + 256 * l);
-    HOLD_LAUNCH_CHECK(ctx);
-  }
-  for (int l = 0; l < 4; ++l) {
-    const int K = (l == 0) ? rgb->in_dim[0] : 256, kpad = (l == 0) ? 320 : 256;
-    t.rgb_nst[l] = kpad / 32;
-    if (!t.rgb_img[l]) HOLD_CUDA(cudaMalloc((void**)&t.rgb_img[l], (size_t)t.rgb_nst[l] * kTcStageBytes));
-    k_tc_pack<<<256, 128, 0, s>>>(rgb->weight_v[l], rgb->weight_g[l], rgb->in_dim[l], 0, 256, K, kpad, 1.0f, l == 0 ? 14 : 0, t.rgb_img[l]);
-    HOLD_LAUNCH_CHECK(ctx);
-  }
-  return HOLD_OK;
+// TcArgs::L[] and the head of a packed net's forward chain.  The images have 256 output rows (zero beyond N); the kernel reads
+// N only at the skip layer, where the embedding columns start, so the colour nets run their layers at the full 256.
+static void tc_layers(const PackedNet& m, bool skip_net, TcArgs& a) {
+  for (int l = 0; l < m.n_layers; ++l)
+    a.L[l].wimg = m.img[l], a.L[l].bias = m.bias_s + 256 * l, a.L[l].nst = m.nst[l], a.L[l].N = skip_net ? m.N[l] : 256;
+  a.w_last = m.w_last_tc ? m.w_last_tc : m.w_last, a.b_last = m.b_last;
 }
 
 // SDF net on P canonical points: sdf only (sampler rounds: 8 layers, sdf head), or sdf + d sdf / d x_c + 256-d feature
 // (reverse mode: 8 forward layers, feature layer, 8 backward layers over the transposed images).
-static int tc_launch_sdf(hold_ctx* ctx, NodeState& ns, int P, const float* xc, const float* embed_w, float* sdf, float* grad,
+static int tc_launch_sdf(hold_ctx* ctx, const PackedNet& net, int P, const float* xc, const float* embed_w, float* sdf, float* grad,
                          float* feat, const SamplerState* st, cudaStream_t s) {
   const bool rev = (grad != nullptr) || (feat != nullptr);
   TcArgs a;
   memset(&a, 0, sizeof(a));
   a.P = P, a.n_layers = rev ? 17 : 8;
-  for (int l = 0; l < 9; ++l) {
-    a.L[l].wimg = ns.tc->sdf_img[l], a.L[l].bias = ns.tc->bias_s + 256 * l, a.L[l].nst = ns.tc->sdf_nst[l], a.L[l].N = ns.sdf.N[l];
-  }
-  a.w_last = ns.sdf.w_last, a.b_last = ns.sdf.b_last;
+  tc_layers(net, true, a);
   a.xc = xc, a.embed_w = embed_w, a.sdf = sdf, a.grad = grad, a.feat = feat, a.st = st, a.err = ctx->dev_err;
   a.passes = (st != nullptr && ctx->sampler_passes >= 1 && ctx->sampler_passes <= 3) ? ctx->sampler_passes : 3;
   a.unscale = kTcUnscale * (1.0f + (float)(ctx->tc_acc_comp >= 0 ? ctx->tc_acc_comp : kTcAccComp) * (1.0f / 16777216.0f));
@@ -984,11 +925,11 @@ static int tc_launch_sdf(hold_ctx* ctx, NodeState& ns, int P, const float* xc, c
   if (rev) {
     HOLD_REQUIRE(grad != nullptr && feat != nullptr, "sdf eval with gradient needs both grad and feat buffers");
     void* sig = nullptr;
-    int rc = ws_get(ctx, 12 /* WS_SIG */, (size_t)grid * 8 * kTcRows * 256 * sizeof(uint16_t), &sig);
+    int rc = ws_get(ctx, WS_SIG, (size_t)grid * 8 * kTcRows * 256 * sizeof(uint16_t), &sig);
     if (rc) return rc;
     a.sig = (uint16_t*)sig;
     for (int i = 0; i < 8; ++i) {
-      a.L[9 + i].wimg = ns.tc->sdf_imgT[7 - i], a.L[9 + i].bias = nullptr, a.L[9 + i].nst = 8, a.L[9 + i].N = 256;
+      a.L[9 + i].wimg = net.imgT[7 - i], a.L[9 + i].bias = nullptr, a.L[9 + i].nst = 8, a.L[9 + i].N = 256;
     }
     k_mlp_tc<MLP_SDF_REV><<<grid, kTcThreadsTotal, TcCfg<MLP_SDF_REV>::kSmemBytes, s>>>(a);
   } else {
@@ -1015,17 +956,14 @@ static int tc_launch_linear_img(hold_ctx* ctx, const uint8_t* img, const float* 
   return HOLD_OK;
 }
 
-static int tc_launch_rgb(hold_ctx* ctx, NodeState& ns, int P, int pts_per_frame, const float* xc, const float* normal,
+static int tc_launch_rgb(hold_ctx* ctx, const PackedNet& net, int P, int pts_per_frame, const float* xc, const float* normal,
                          const float* pe, const float* feat, const float* time_code, float* rgb, cudaStream_t s) {
   TcArgs a;
   memset(&a, 0, sizeof(a));
-  a.P = P, a.n_layers = 4;
-  for (int l = 0; l < 4; ++l) {
-    a.L[l].wimg = ns.tc->rgb_img[l], a.L[l].bias = ns.tc->bias_s + 256 * (9 + l), a.L[l].nst = ns.tc->rgb_nst[l], a.L[l].N = 256;
-  }
-  a.w_last = ns.rgb.w_last, a.b_last = ns.rgb.b_last;
+  a.P = P, a.n_layers = net.n_layers;
+  tc_layers(net, false, a);
   a.xc = xc, a.normal = normal, a.pose_embed = pe, a.feat = const_cast<float*>(feat), a.time_code = time_code;
-  a.pts_per_frame = pts_per_frame, a.k0 = ns.rgb.K[0], a.rgb = rgb, a.err = ctx->dev_err, a.unscale = kTcUnscale, a.passes = 3;
+  a.pts_per_frame = pts_per_frame, a.k0 = net.K[0], a.rgb = rgb, a.err = ctx->dev_err, a.unscale = kTcUnscale, a.passes = 3;
   int tiles = ceil_div(P, kTcRows);
   k_mlp_tc<MLP_COLOR><<<min(tiles, ctx->sm_count), kTcThreadsTotal, TcCfg<MLP_COLOR>::kSmemBytes, s>>>(a);
   HOLD_LAUNCH_CHECK(ctx);

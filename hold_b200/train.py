@@ -43,7 +43,7 @@ def _ld(t):
     return t.stride(0)
 
 
-def _ew(node, op, P, ncols, in0, in1=None, in2=None, out0=None, out1=None, aux=0, ld2=None):
+def _ew(ctx, op, P, ncols, in0, in1=None, in2=None, out0=None, out1=None, aux=0, ld2=None):
     a = EwArgs()
     a.in0, a.in1, a.in2 = in0.data_ptr(), (in1.data_ptr() if in1 is not None else None), (in2.data_ptr() if in2 is not None else None)
     a.out0, a.out1 = out0.data_ptr(), (out1.data_ptr() if out1 is not None else None)
@@ -53,16 +53,21 @@ def _ew(node, op, P, ncols, in0, in1=None, in2=None, out0=None, out1=None, aux=0
     a.ld_out0 = _ld(out0)
     a.ld_out1 = _ld(out1) if out1 is not None else 0
     a.ncols, a.aux = ncols, aux
-    check(lib().hold_train_ew(node.ctx.h, op, P, C.byref(a), stream_ptr()))
+    check(lib().hold_train_ew(ctx.h, op, P, C.byref(a), stream_ptr()))
+
+
+RGB_LEAD, BG_RGB_LEAD = 14, 59   # colour lin0 inputs before the 256 features: [x_c, n, pose embed] / [view PE-4, frame code]
 
 
 class CudaOps:
-    """train_algo backend on libhold_b200.so.  net = "sdf" | "rgb".  Activations live in [P,256] (or [P,320]) row buffers."""
+    """train_algo backend on libhold_b200.so for one net of node slot `slot` (-1: the background's nets).  W, b: the folded fp32
+    tensors (detached) in the reference's column order; the packed matrices' shapes follow from them.  lead = None: a skip net
+    (SDF net, background implicit net); else a colour net whose lin0 has `lead` inputs before the 256 features.  Activations live
+    in [P,256] (or [P,320]) row buffers."""
 
-    def __init__(self, node, net, W, b):
-        self.node, self.net, self.W, self.b = node, net, W, b   # W, b: folded fp32 tensors (detached), reference column order
+    def __init__(self, ctx, slot, W, b, lead=None):
+        self.ctx, self.slot, self.W, self.b, self.lead = ctx, slot, W, b, lead
         self.scaled = False                                       # backward: scale operands by a power of two (hold_linear in_scale)
-        self.hand = node.kind == "hand"
 
     # ---- products with a weight matrix
     def _linear(self, mat, A, kvalid, nvalid, bias, out_cols=256):
@@ -70,48 +75,51 @@ class CudaOps:
         assert A.stride(1) == 1 and A.stride(0) % 4 == 0 and A.data_ptr() % 16 == 0, "hold_linear wants 16-byte aligned rows"
         out = torch.empty(P, out_cols, device=A.device)
         sc = self._scale(A) if self.scaled else None
-        check(lib().hold_linear(self.node.ctx.h, self.node.slot, mat, P, ptr(A) if A.is_contiguous() else C.c_void_p(A.data_ptr()), A.stride(0),
+        check(lib().hold_linear(self.ctx.h, self.slot, mat, P, ptr(A) if A.is_contiguous() else C.c_void_p(A.data_ptr()), A.stride(0),
                                 kvalid, 1 if bias else 0, ptr(sc), C.c_void_p(out.data_ptr()), out.stride(0), nvalid, stream_ptr()))
         return out[:, :nvalid]
 
     def _scale(self, t):
         """device scalar 2^floor(log2 max|t|) (hold_pow2_scale: two small launches, no host sync)"""
         sc = torch.empty(1, device=t.device)
-        check(lib().hold_pow2_scale(self.node.ctx.h, t.shape[0], t.shape[1], C.c_void_p(t.data_ptr()), t.stride(0), ptr(sc), stream_ptr()))
+        check(lib().hold_pow2_scale(self.ctx.h, t.shape[0], t.shape[1], C.c_void_p(t.data_ptr()), t.stride(0), ptr(sc), stream_ptr()))
         return sc
 
     def lin(self, A, l, bias=True):
-        if self.net == "sdf":
+        if self.lead is None:
             if l == 8:   # [sdf head | 256 feature rows]: the head is a matrix-vector product
-                feat = self._linear(8, A, 256, 256, bias)
+                feat = self._linear(capi.MAT_SKIP_W + 8, A, 256, 256, bias)
                 head = A @ self.W[8][0] + (self.b[8][0] if bias else 0.0)
                 return torch.cat([head[:, None], feat], 1)
-            n = T.N_SKIP_A if l == 3 else 256
-            return self._linear(l, A, A.shape[1], n, bias)
-        if l == 4:       # 3-row sigmoid head
-            y = A @ self.W[4].T
-            return y + self.b[4] if bias else y
-        if l == 0:       # kernel operand order: [feature (256) | x_c, n, pose (14) | time code (32)]
-            A = torch.cat([A[:, 14:270], A[:, :14], A[:, 270:], A.new_zeros(A.shape[0], 320 - A.shape[1])], 1)
-            return self._linear(32, A, 320, 256, bias)
-        return self._linear(32 + l, A, 256, 256, bias)
+            return self._linear(capi.MAT_SKIP_W + l, A, A.shape[1], self.W[l].shape[0], bias)
+        width = self.W[0].shape[0]
+        if l == len(self.W) - 1:   # 3-row sigmoid head
+            y = A @ self.W[l].T
+            return y + self.b[l] if bias else y
+        if l == 0:       # kernel operand order: [feature (256) | the lead inputs | the inputs after the features], padded to 320
+            ld = self.lead
+            A = torch.cat([A[:, ld:ld + 256], A[:, :ld], A[:, ld + 256:], A.new_zeros(A.shape[0], 320 - A.shape[1])], 1)
+            return self._linear(capi.MAT_COLOUR_W, A, 320, width, bias)
+        return self._linear(capi.MAT_COLOUR_W + l, A, width, width, bias)
 
     def lin_t(self, A, l):
-        if self.net == "sdf":
+        if self.lead is None:
             if l == 8:
                 d_feat = A[:, 1:].contiguous()
-                return A[:, :1] * self.W[8][0][None, :] + self._linear(24, d_feat, 256, 256, False)
+                return A[:, :1] * self.W[8][0][None, :] + self._linear(capi.MAT_SKIP_WT + 8, d_feat, 256, 256, False)
             if l == 0:
-                return self._linear(16, A, 256, T.D_EMBED, False, out_cols=40)
-            return self._linear(16 + l, A, A.shape[1], 256, False)
-        if l == 4:
-            return A @ self.W[4]
+                k_in = self.W[0].shape[1]
+                return self._linear(capi.MAT_SKIP_WT, A, 256, k_in, False, out_cols=(k_in + 3) // 4 * 4)
+            return self._linear(capi.MAT_SKIP_WT + l, A, A.shape[1], 256, False)
+        width = self.W[0].shape[0]
+        if l == len(self.W) - 1:
+            return A @ self.W[l]
         if l == 0:
-            k0 = self.W[0].shape[1]
-            f = self._linear(48, A, 256, 256, False)
-            o = self._linear(49, A, 256, 64, False, out_cols=64)
-            return torch.cat([o[:, :14], f, o[:, 14:14 + (k0 - 270)]], 1)
-        return self._linear(49 + l, A, 256, 256, False)
+            ld, k0 = self.lead, self.W[0].shape[1]
+            f = self._linear(capi.MAT_COLOUR_WT, A, width, 256, False)
+            o = self._linear(capi.MAT_COLOUR_WT + 1, A, width, 64, False, out_cols=64)
+            return torch.cat([o[:, :ld], f, o[:, ld:k0 - 256]], 1)
+        return self._linear(capi.MAT_COLOUR_WT + 1 + l, A, width, width, False)
 
     def wgrad(self, D, A):
         """D^T A over the points: hold_wgrad (tensor cores, operands rescaled by powers of two) in blocks of <= 256 x 256."""
@@ -124,7 +132,7 @@ class CudaOps:
         sd, sa = self._scale(D), self._scale(A)
         for n0 in range(0, N, 256):
             for k0 in range(0, K, 256):
-                check(lib().hold_wgrad(self.node.ctx.h, P, C.c_void_p(D.data_ptr() + 4 * n0), D.stride(0), min(256, N - n0),
+                check(lib().hold_wgrad(self.ctx.h, P, C.c_void_p(D.data_ptr() + 4 * n0), D.stride(0), min(256, N - n0),
                                        C.c_void_p(A.data_ptr() + 4 * k0), A.stride(0), min(256, K - k0), ptr(sd), ptr(sa),
                                        C.c_void_p(out.data_ptr() + 4 * (n0 * K + k0)), K, stream_ptr()))
         return out
@@ -139,14 +147,14 @@ class CudaOps:
     def act(self, z, e=None):
         P, n = z.shape
         a, s = torch.empty(P, 256, device=z.device), torch.empty(P, 256, device=z.device)
-        _ew(self.node, EW["ACT"], P, n, z, e, None, a, s, aux=0 if e is None else e.shape[1])
+        _ew(self.ctx, EW["ACT"], P, n, z, e, None, a, s, aux=0 if e is None else e.shape[1])
         return (a[:, :n] if e is None else a[:, :n + e.shape[1]]), s[:, :n]
 
     def _binary(self, op, x, y, in2=None, ld2=None, two=False):
         P, n = y.shape
         o0 = torch.empty(P, 256 if n <= 256 else 320, device=y.device)
         o1 = torch.empty_like(o0) if two else None
-        _ew(self.node, op, P, n, x, y, in2, o0, o1, ld2=ld2)
+        _ew(self.ctx, op, P, n, x, y, in2, o0, o1, ld2=ld2)
         return (o0[:, :n], o1[:, :n]) if two else o0[:, :n]
 
     def mul(self, x, y):
@@ -167,25 +175,25 @@ class CudaOps:
         P = x.shape[0]
         out = torch.empty(P, 40, device=x.device)
         xc = x.contiguous()
-        _ew(self.node, EW["EMBED"], P, 40, xc, embed_w, None, out, aux=order)
+        _ew(self.ctx, EW["EMBED"], P, 40, xc, embed_w, None, out, aux=order)
         return out[:, :T.D_EMBED]
 
     def embed_vjp(self, d1, ge):
         P = d1.shape[0]
         out = torch.empty(P, 3, device=d1.device)
-        _ew(self.node, EW["EMBED_VJP"], P, 3, d1, ge, None, out)
+        _ew(self.ctx, EW["EMBED_VJP"], P, 3, d1, ge, None, out)
         return out
 
     def embed_jvp(self, d1, v):
         P = d1.shape[0]
         out = torch.empty(P, 40, device=d1.device)
-        _ew(self.node, EW["EMBED_JVP"], P, 40, d1, v.contiguous(), None, out)
+        _ew(self.ctx, EW["EMBED_JVP"], P, 40, d1, v.contiguous(), None, out)
         return out[:, :T.D_EMBED]
 
     def relu(self, z):
         P, n = z.shape
         out = torch.empty(P, 256, device=z.device)
-        _ew(self.node, EW["RELU"], P, n, z, None, None, out)
+        _ew(self.ctx, EW["RELU"], P, n, z, None, None, out)
         return out[:, :n]
 
     def relu_bwd(self, dA, a):
@@ -214,7 +222,7 @@ class SdfNetFn(torch.autograd.Function):
         W, b = [w.detach().float() for w in Wb[:9]], [v.detach().float() for v in Wb[9:]]
         Wk = list(W)
         Wk[0] = W[0][:, :T.D_EMBED].contiguous()     # hand: the 45 pose-condition columns are multiplied by zero (shape_net.py:104-106)
-        ops = CudaOps(node, "sdf", Wk, b)
+        ops = CudaOps(node.ctx, node.slot, Wk, b)
         sdf, feat, g, st = T.sdf_forward(ops, x.detach().float().contiguous(), node.embed_w())
         fctx.ops, fctx.st, fctx.k0 = ops, st, W[0].shape[1]
         return sdf.contiguous(), feat.contiguous(), g
@@ -225,7 +233,7 @@ class SdfNetFn(torch.autograd.Function):
         ops.scaled = True
         f = lambda t: None if t is None else t.float().contiguous()
         d_x, dW, db = T.sdf_backward(ops, fctx.st, f(d_sdf), f(d_feat), f(d_g))
-        dW[4] = dW[4] * (1.0 / math.sqrt(2.0))       # the packed W_4 carries the skip's 1/sqrt 2
+        dW[4] = dW[4] * T.SQ2       # the packed W_4 carries the skip's 1/sqrt 2
         if fctx.k0 > T.D_EMBED:
             dW[0] = torch.cat([dW[0], dW[0].new_zeros(256, fctx.k0 - T.D_EMBED)], 1)
         return (None, d_x, *dW, *db)
@@ -238,7 +246,7 @@ class RgbNetFn(torch.autograd.Function):
     @staticmethod
     def forward(fctx, node, inp, *Wb):
         W, b = [w.detach().float() for w in Wb[:5]], [v.detach().float() for v in Wb[5:]]
-        ops = CudaOps(node, "rgb", W, b)
+        ops = CudaOps(node.ctx, node.slot, W, b, lead=RGB_LEAD)
         rgb, st = T.rgb_forward(ops, inp.detach().float().contiguous())
         fctx.ops, fctx.st = ops, st
         return rgb
@@ -370,53 +378,13 @@ def merge_factors(fl):
 
 
 # ------------------------------------------------------------------------------------------------ background (renderables/background.py)
-class _BgHandle:
-    """What CudaOps needs from a "node" when the matrices are the background's (hold_linear with node = -1)."""
-
-    def __init__(self, ctx):
-        self.ctx, self.slot, self.kind = ctx, -1, "background"
-
-
-class BgOps(CudaOps):
-    """train_algo backend for the background nets: net = "bg_sdf" (9 plain layers, 116 inputs, skip at 4) | "bg_rgb" (315 -> 128 -> 3)."""
-
-    def __init__(self, ctx, net, W, b):
-        super().__init__(_BgHandle(ctx), net, W, b)
-
-    def lin(self, A, l, bias=True):
-        if self.net == "bg_sdf":
-            if l == 8:
-                feat = self._linear(8, A, 256, 256, bias)
-                head = A @ self.W[8][0] + (self.b[8][0] if bias else 0.0)
-                return torch.cat([head[:, None], feat], 1)
-            return self._linear(l, A, A.shape[1], 172 if l == 3 else 256, bias)
-        if l == 1:       # 128 -> 3 head
-            y = A @ self.W[1].T
-            return y + self.b[1] if bias else y
-        A = torch.cat([A[:, 59:], A[:, :59], A.new_zeros(A.shape[0], 5)], 1)      # operand order [feature (256) | view, frame (59)] + pad
-        return self._linear(32, A, 320, 128, bias)
-
-    def lin_t(self, A, l):
-        if self.net == "bg_sdf":
-            if l == 8:
-                return A[:, :1] * self.W[8][0][None, :] + self._linear(24, A[:, 1:].contiguous(), 256, 256, False)
-            if l == 0:
-                return self._linear(16, A, 256, 116, False, out_cols=116)
-            return self._linear(16 + l, A, A.shape[1], 256, False)
-        if l == 1:
-            return A @ self.W[1]
-        f = self._linear(48, A, 128, 256, False)
-        o = self._linear(49, A, 128, 64, False, out_cols=64)
-        return torch.cat([o[:, :59], f], 1)
-
-
 class BgSdfFn(torch.autograd.Function):
     """out [P,257] = bg_implicit_network([PE-10(point) | frame code]); differentiable w.r.t. the input rows (frame code) and weights."""
 
     @staticmethod
     def forward(fctx, ctx, inp, *Wb):
         W, b = [w.detach().float() for w in Wb[:9]], [v.detach().float() for v in Wb[9:]]
-        ops = BgOps(ctx, "bg_sdf", W, b)
+        ops = CudaOps(ctx, -1, W, b)
         out, st = T.skipnet_forward(ops, inp.detach().float().contiguous(), skip=4, d_skip=84)
         fctx.ops, fctx.st = ops, st
         return out
@@ -425,7 +393,7 @@ class BgSdfFn(torch.autograd.Function):
     def backward(fctx, d_out):
         fctx.ops.scaled = True
         d_inp, dW, db = T.skipnet_backward(fctx.ops, fctx.st, d_out.float().contiguous())
-        dW[4] = dW[4] * (1.0 / math.sqrt(2.0))
+        dW[4] = dW[4] * T.SQ2
         return (None, d_inp, *dW, *db)
 
 
@@ -434,7 +402,7 @@ class BgRgbFn(torch.autograd.Function):
 
     @staticmethod
     def forward(fctx, ctx, inp, W0, W1, b0, b1):
-        ops = BgOps(ctx, "bg_rgb", [W0.detach().float(), W1.detach().float()], [b0.detach().float(), b1.detach().float()])
+        ops = CudaOps(ctx, -1, [W0.detach().float(), W1.detach().float()], [b0.detach().float(), b1.detach().float()], lead=BG_RGB_LEAD)
         rgb, st = T.head_forward(ops, inp.detach().float().contiguous())
         fctx.ops, fctx.st = ops, st
         return rgb

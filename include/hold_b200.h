@@ -251,7 +251,7 @@ int hold_render_fg(hold_ctx* ctx, int n, const int32_t* node_ids_host, int R, in
                    int32_t* iters /*[n] device*/, void* stream);
 
 /* SURVEY §8f rank 1 — the NeRF++ background (model/renderables/background.py).
- * hold_bg_set_weights: Background.bg_implicit_network (9 plain layers `lin<k>.{weight,bias}`: weight_g NULL) and
+ * hold_bg_set_weights: Background.bg_implicit_network (9 plain layers `lin<k>.{weight,bias}`: weight_g NULL, else HOLD_E_BADARG) and
  * Background.bg_rendering_network (2 plain layers, 315 -> 128 -> 3); mlp_mode = HOLD_MLP_* arithmetic of both nets.
  * hold_background: HOLDNet.forward's background leg (hold/hold_net.py:91-118,125-134): inverse_sample +
  * Background.forward.  fg_bg_weights [R] is volumetric_render's `bg_weights`; frame_code [B,32] is
@@ -280,7 +280,8 @@ int hold_rgb_eval(hold_ctx* ctx, int node, int B, int P, const float* x_c, const
  *    16..24  SDF W_l^T (A has N_l columns, C has K_l: 39 for l = 0)
  *    32..35  colour W_l, l = 0..3 (texture_net.py:95-100); l = 0 takes A in the order [feature (256) | x_c, n, pose (14) | time code (32)]
  *    48, 49  colour W_0^T: to the 256 feature inputs / to the other inputs [x_c, n, pose (14) | time code (32)];  50..52  colour W_1..3^T
- * node = -1 addresses the background nets (model/renderables/background.py; packed by hold_bg_set_weights with HOLD_MLP_TC): 0..8 the
+ * node = -1 addresses the background nets (model/renderables/background.py; packed by hold_bg_set_weights with HOLD_MLP_TC, HOLD_E_STATE
+ * if they were last packed with HOLD_MLP_FP32): 0..8 the
  * implicit net's W_l (lin0: 116 inputs = PE-10 of the 4-d point (84) + frame code (32); lin3: 172 outputs, the skip re-feeds the 84 embedding columns), 16..24 their transposes, 32 the colour
  * head's lin0 (315 -> 128, A in the order [feature (256) | view PE-4 (27), frame code (32)]), 48 / 49 its transpose to the features / to
  * [view, frame code].
