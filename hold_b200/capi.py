@@ -97,6 +97,9 @@ EXPORTS = {
     "hold_render_fg": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.c_int, C.c_int, fp, fp, C.POINTER(NodePose), C.POINTER(Factors), C.POINTER(RenderOut), C.POINTER(RenderOut), fp, C.c_void_p]),
     "hold_bg_set_weights": (C.c_int, [C.c_void_p, C.POINTER(MlpWeights), C.POINTER(MlpWeights), C.c_int, C.c_void_p]),
     "hold_background": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, fp, fp, fp, fp, fp, fp, C.c_void_p]),
+    "hold_bg_encode": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, fp, fp, fp, C.c_int, fp, C.c_int, C.c_void_p]),
+    "hold_bg_integrate": (C.c_int, [C.c_void_p, C.c_int, fp, fp, fp, fp, fp, fp, fp, C.c_void_p]),
+    "hold_bg_integrate_bwd": (C.c_int, [C.c_void_p, C.c_int, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, C.c_void_p]),
     "hold_sdf_eval": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, fp, fp, fp, C.c_void_p]),
     "hold_linear": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, fp, C.c_int, C.c_int, C.c_int, fp, fp, C.c_int, C.c_int, C.c_void_p]),
     "hold_wgrad": (C.c_int, [C.c_void_p, C.c_int, fp, C.c_int, C.c_int, fp, C.c_int, C.c_int, fp, fp, fp, C.c_int, C.c_void_p]),

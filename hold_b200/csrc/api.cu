@@ -1080,6 +1080,15 @@ int hold_bg_set_weights(hold_ctx* ctx, const hold_mlp_weights* sdf, const hold_m
   return HOLD_OK;
 }
 
+// the bounding sphere is a per-node constant in the reference (same value for all nodes): take the first configured node's
+static int bg_sphere(hold_ctx* ctx, float* r_sphere) {
+  *r_sphere = 0.f;
+  for (int n = 0; n < HOLD_MAX_NODES; ++n)
+    if (ctx->nodes[n].configured) { *r_sphere = ctx->nodes[n].cfg.bounding_sphere; break; }
+  HOLD_REQUIRE(*r_sphere > 0.f, "configure a node first (scene_bounding_sphere)");
+  return HOLD_OK;
+}
+
 int hold_background(hold_ctx* ctx, int R, int B, const float* cam_loc, const float* ray_dirs, const float* frame_code,
                     const float* fg_bg_weights, float* bg_rgb, float* bg_rgb_only, float* bg_semantics, float* bg_z_vals,
                     void* stream) {
@@ -1090,6 +1099,8 @@ int hold_background(hold_ctx* ctx, int R, int B, const float* cam_loc, const flo
   if (R == 0) return HOLD_OK;
   HOLD_REQUIRE(R % B == 0, "R (%d) must be B (%d) frames x rays, frame-major", R, B);
   HOLD_REQUIRE(cam_loc && ray_dirs && frame_code && fg_bg_weights, "NULL argument");
+  float r_sphere;
+  if (int rc = bg_sphere(ctx, &r_sphere)) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   const int rpf = R / B;
   const int rays_per_chunk = max(1, min(rpf, (1 << 20) / kBgN));
@@ -1104,11 +1115,7 @@ int hold_background(hold_ctx* ctx, int R, int B, const float* cam_loc, const flo
       BgArgs a;
       memset(&a, 0, sizeof(a));
       a.P = P, a.pts_per_frame = P, a.cam = cam_loc + ray0 * 3, a.dirs = ray_dirs + ray0 * 3, a.frame_code = frame_code + (size_t)b * kBgFrame;
-      a.r_sphere = 0.f;
-      // the bounding sphere is a per-node constant in the reference (same value for all nodes): take node 0's
-      for (int n = 0; n < HOLD_MAX_NODES; ++n)
-        if (ctx->nodes[n].configured) { a.r_sphere = ctx->nodes[n].cfg.bounding_sphere; break; }
-      HOLD_REQUIRE(a.r_sphere > 0.f, "configure a node first (scene_bounding_sphere)");
+      a.r_sphere = r_sphere;
       simt_layers(ctx->bg_sdf, ctx->bg_sdf.n_layers, a);
       a.sdf = sdf_ws, a.feat = feat_ws;
       if (ctx->bg_mlp_mode == HOLD_MLP_TC) {
@@ -1124,12 +1131,57 @@ int hold_background(hold_ctx* ctx, int R, int B, const float* cam_loc, const flo
         k_bg_mlp<BG_RGB><<<min(tiles, ctx->sm_count), 256, kBgSmemBytes, s>>>(c);
         HOLD_LAUNCH_CHECK(ctx);
       }
-      k_bg_composite<<<ceil_div(rn, 128), 128, 0, s>>>(rn, a.r_sphere, sdf_ws, rgb_ws, fg_bg_weights + ray0,
+      k_bg_composite<<<ceil_div(rn, 128), 128, 0, s>>>(rn, a.r_sphere, nullptr, sdf_ws, rgb_ws, fg_bg_weights + ray0,
                                                        bg_rgb ? bg_rgb + ray0 * 3 : nullptr, bg_rgb_only ? bg_rgb_only + ray0 * 3 : nullptr,
                                                        bg_semantics ? bg_semantics + ray0 * 4 : nullptr, bg_z_vals ? bg_z_vals + ray0 * kBgN : nullptr);
       HOLD_LAUNCH_CHECK(ctx);
     }
   }
+  return HOLD_OK;
+}
+
+int hold_bg_encode(hold_ctx* ctx, int R, int B, const float* cam_loc, const float* ray_dirs, const float* jitter, float* bg_z_vals,
+                   float* pe_pts, int ld_pts, float* pe_view, int ld_view, void* stream) {
+  HOLD_REQUIRE(ctx != nullptr, "ctx is NULL");
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  HOLD_REQUIRE(R >= 0 && B >= 1, "bad R/B");
+  HOLD_REQUIRE(R % B == 0, "R (%d) must be B (%d) frames x rays, frame-major", R, B);
+  HOLD_REQUIRE(ld_pts >= kBgEmbed && ld_view >= kBgView, "ld_pts (%d) must be >= %d and ld_view (%d) >= %d", ld_pts, kBgEmbed, ld_view, kBgView);
+  HOLD_REQUIRE((size_t)R * kBgN <= (size_t)INT32_MAX, "R (%d) too large", R);
+  if (R == 0) return HOLD_OK;
+  HOLD_REQUIRE(cam_loc && ray_dirs && bg_z_vals && pe_pts && pe_view, "NULL argument");
+  float r_sphere;
+  if (int rc = bg_sphere(ctx, &r_sphere)) return rc;
+  k_bg_encode<<<ceil_div(R * kBgN, 128), 128, 0, (cudaStream_t)stream>>>(R, r_sphere, cam_loc, ray_dirs, jitter, bg_z_vals, pe_pts, ld_pts,
+                                                                        pe_view, ld_view);
+  HOLD_LAUNCH_CHECK(ctx);
+  return HOLD_OK;
+}
+
+int hold_bg_integrate(hold_ctx* ctx, int R, const float* bg_z_vals, const float* sdf, const float* rgb, const float* fg_bg_weights,
+                      float* bg_rgb, float* bg_rgb_only, float* bg_semantics, void* stream) {
+  HOLD_REQUIRE(ctx != nullptr, "ctx is NULL");
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  HOLD_REQUIRE(R >= 0, "negative R");
+  if (R == 0) return HOLD_OK;
+  HOLD_REQUIRE(bg_z_vals && sdf && rgb && fg_bg_weights, "NULL argument");
+  k_bg_composite<<<ceil_div(R, 128), 128, 0, (cudaStream_t)stream>>>(R, 0.f, bg_z_vals, sdf, rgb, fg_bg_weights, bg_rgb, bg_rgb_only,
+                                                                    bg_semantics, nullptr);
+  HOLD_LAUNCH_CHECK(ctx);
+  return HOLD_OK;
+}
+
+int hold_bg_integrate_bwd(hold_ctx* ctx, int R, const float* bg_z_vals, const float* sdf, const float* rgb, const float* fg_bg_weights,
+                          const float* g_bg_rgb, const float* g_bg_rgb_only, const float* g_bg_semantics, float* d_sdf, float* d_rgb,
+                          float* d_fg_bg_weights, void* stream) {
+  HOLD_REQUIRE(ctx != nullptr, "ctx is NULL");
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  HOLD_REQUIRE(R >= 0 && R <= INT32_MAX / kBgN, "bad R (%d)", R);
+  if (R == 0) return HOLD_OK;
+  HOLD_REQUIRE(bg_z_vals && sdf && rgb && fg_bg_weights && d_sdf && d_rgb && d_fg_bg_weights, "NULL argument");
+  k_bg_composite_bwd<<<ceil_div(R * kBgN, 128), 128, 0, (cudaStream_t)stream>>>(R, bg_z_vals, sdf, rgb, fg_bg_weights, g_bg_rgb, g_bg_rgb_only,
+                                                                               g_bg_semantics, d_sdf, d_rgb, d_fg_bg_weights);
+  HOLD_LAUNCH_CHECK(ctx);
   return HOLD_OK;
 }
 

@@ -183,30 +183,87 @@ __global__ void __launch_bounds__(256, 1) k_bg_mlp(BgArgs a) {
 }
 constexpr size_t kBgSmemBytes = (size_t)(2 * kTileRows * kBgActLd + 2 * kKC * 256 + kTileRows * kBgEmbLd) * sizeof(float);
 
-// bg_volume_rendering (background.py:137-165) over the flipped depths + Background.forward's outputs (:35-54)
-__global__ void k_bg_composite(int R, float r_sphere, const float* __restrict__ sdf /*[R,32]*/,
+// inverse_sample (ray_sampler.py:82-85, stratified when `jitter` [R,32] is given) + the per-sample inputs of Background.forward
+// (background.py:56-100), one thread per (ray, flipped sample k), row p = ray * 32 + k: bg_z_vals [R,32] un-flipped, as
+// inverse_sample returns it; PE-10 of depth2pts_outside -> pe_pts rows (84 columns); PE-4 of the view direction -> pe_view (27).
+__global__ void __launch_bounds__(128) k_bg_encode(int R, float r_sphere, const float* __restrict__ cam, const float* __restrict__ dirs,
+                                                   const float* __restrict__ jitter, float* __restrict__ z_out, float* __restrict__ pe_pts,
+                                                   int ld_pts, float* __restrict__ pe_view, int ld_view) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= R * kBgN) return;
+  const int ray = p / kBgN, k = p % kBgN;
+  const size_t zi = (size_t)ray * kBgN + (kBgN - 1 - k);
+  const float depth = bg_depth(k, r_sphere, jitter ? jitter + zi : nullptr);
+  z_out[zi] = depth;
+  const float o[3] = {cam[3 * ray], cam[3 * ray + 1], cam[3 * ray + 2]};
+  const float d[3] = {dirs[3 * ray], dirs[3 * ray + 1], dirs[3 * ray + 2]};
+  float p4[4];
+  depth2pts_outside(o, d, depth, r_sphere, p4);
+  embed_generic<4, 10>(p4, pe_pts + (size_t)p * ld_pts);
+  embed_generic<3, 4>(d, pe_view + (size_t)p * ld_view);
+}
+
+// bg_volume_rendering (background.py:137-165) over the flipped depths + Background.forward's outputs (:35-54).  z: the un-flipped
+// depths [R,32] of hold_bg_encode, or NULL for the fixed shells (then z_bg, if given, receives them).
+__global__ void k_bg_composite(int R, float r_sphere, const float* __restrict__ z, const float* __restrict__ sdf /*[R,32]*/,
                                const float* __restrict__ rgb /*[R,32,3]*/, const float* __restrict__ fg_bg_weights /*[R]*/,
                                float* __restrict__ bg_rgb, float* __restrict__ bg_rgb_only, float* __restrict__ bg_sem,
                                float* __restrict__ z_bg) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= R) return;
-  float cum = 0.f, acc[3] = {0.f, 0.f, 0.f};
-  for (int k = 0; k < kBgN; ++k) {
-    const float zk = bg_depth(k, r_sphere);
-    const float dist = (k + 1 < kBgN) ? zk - bg_depth(k + 1, r_sphere) : 1.0e10f;
-    const float fe = dist * fabsf(sdf[(size_t)r * kBgN + k]);   // AbsDensity
-    const float w = (1.0f - expf(-fe)) * expf(-cum);
-    cum += fe;
-    const float* c = rgb + ((size_t)r * kBgN + k) * 3;
-    acc[0] += w * c[0], acc[1] += w * c[1], acc[2] += w * c[2];
-    if (z_bg != nullptr) z_bg[(size_t)r * kBgN + (kBgN - 1 - k)] = zk;  // un-flipped, as inverse_sample returns it
-  }
+  float acc[3];
+  bg_integrate_ray(z ? z + (size_t)r * kBgN : nullptr, r_sphere, sdf + (size_t)r * kBgN, rgb + (size_t)r * kBgN * 3, acc);
+  if (z_bg != nullptr)
+    for (int k = 0; k < kBgN; ++k) z_bg[(size_t)r * kBgN + (kBgN - 1 - k)] = bg_depth(k, r_sphere);
   const float wbg = fg_bg_weights[r];
   for (int c = 0; c < 3; ++c) {
     if (bg_rgb_only) bg_rgb_only[3 * r + c] = acc[c];
     if (bg_rgb) bg_rgb[3 * r + c] = wbg * acc[c];
   }
   if (bg_sem) { bg_sem[4 * r] = wbg; bg_sem[4 * r + 1] = 0.f; bg_sem[4 * r + 2] = 0.f; bg_sem[4 * r + 3] = 0.f; }
+}
+
+// reverse mode of k_bg_composite w.r.t. sdf, rgb and fg_bg_weights (bg_phases.h), one warp per ray, lane k = flipped sample k:
+// the transmittance is an exclusive prefix sum over the lanes, sum_{i>k} d w_i w_i an exclusive suffix sum.
+__global__ void __launch_bounds__(128) k_bg_composite_bwd(int R, const float* __restrict__ z, const float* __restrict__ sdf,
+                                                          const float* __restrict__ rgb, const float* __restrict__ fg_bg_weights,
+                                                          const float* __restrict__ g_rgb, const float* __restrict__ g_only,
+                                                          const float* __restrict__ g_sem, float* __restrict__ d_sdf,
+                                                          float* __restrict__ d_rgb, float* __restrict__ d_wfg) {
+  static_assert(kBgN == 32, "one lane per sample");
+  const int r = (blockIdx.x * blockDim.x + threadIdx.x) / 32, k = threadIdx.x % 32;
+  if (r >= R) return;
+  const size_t p = (size_t)r * kBgN + k;
+  const float dist = bg_interval(z + (size_t)r * kBgN, 0.f, k);
+  const float s = sdf[p];
+  const float fe = dist * fabsf(s);
+  float incl = fe;   // inclusive prefix sum of fe over the lanes
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (k >= o) incl += v;
+  }
+  // exclusive sums by a shift, not by subtracting the own term: the last interval is 1e10 and would swamp the others
+  float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (k == 0) excl = 0.f;
+  float g[3];
+  bg_bwd_seed(g_rgb ? g_rgb + 3 * r : nullptr, g_only ? g_only + 3 * r : nullptr, fg_bg_weights[r], g);
+  const float* c = rgb + p * 3;
+  const BgSampleBwd b = bg_bwd_sample(fe, excl, c, g, d_rgb + p * 3);
+  float suf = b.dw * b.w;     // inclusive suffix sum of d w_i w_i
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float v = __shfl_down_sync(0xffffffffu, suf, o);
+    if (k + o < 32) suf += v;
+  }
+  float after = __shfl_down_sync(0xffffffffu, suf, 1);
+  if (k == 31) after = 0.f;
+  d_sdf[p] = bg_bwd_dsdf(b, after, dist, s);
+  float only[3] = {b.w * c[0], b.w * c[1], b.w * c[2]};
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+    for (int ch = 0; ch < 3; ++ch) only[ch] += __shfl_xor_sync(0xffffffffu, only[ch], o);
+  if (k == 0) d_wfg[r] = bg_bwd_dwfg(only, g_rgb ? g_rgb + 3 * r : nullptr, g_sem ? g_sem + 4 * r : nullptr);
 }
 
 }  // namespace hold

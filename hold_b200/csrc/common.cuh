@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "../../include/hold_b200.h"
+#include "bg_phases.h"
 
 namespace hold {
 
@@ -112,35 +113,17 @@ int ws_get(hold_ctx* ctx, int slot, size_t bytes, void** out);  // grow-only wor
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline int round_up(int a, int b) { return ceil_div(a, b) * b; }
 
-// torch.linspace(start, end, steps)[i] in fp32 — symmetric evaluation like ATen's linspace kernel
-// (RangeFactories: first half from start, second half from end).
-__host__ __device__ inline float torch_linspace(float start, float end, int steps, int i) {
-  if (steps == 1) return start;
-  float step = (end - start) / (float)(steps - 1);
-  int half = steps / 2;
-  // ATen's linspace kernels (CPU and CUDA) evaluate start + step * i as one fused multiply-add (checked against torch.linspace
-  // bit for bit, tests/test_cpu_host.py); spelled out so that host and device builds agree
-  return (i < half) ? fmaf(step, (float)i, start) : fmaf(-step, (float)(steps - i - 1), end);
-}
-
 // LaplaceDensity.density_func (engine/density.py:21-26)
 __device__ inline float laplace_density(float s, float beta) {
   float sg = (s > 0.f) ? 1.f : ((s < 0.f) ? -1.f : 0.f);
   return (1.0f / beta) * (0.5f + 0.5f * sg * expm1f(-fabsf(s) / beta));
 }
 
-// ---- NeRF++ background geometry (model/renderables/background.py), shared by background.cuh and the tensor-core variant
-constexpr int kBgN = 32;        // N_samples_inverse_sphere
+// ---- NeRF++ background geometry (model/renderables/background.py), shared by background.cuh and the tensor-core variant;
+// the sample depths (kBgN, bg_depth) are in bg_phases.h
 constexpr int kBgEmbed = 84;    // 4 + 4*2*10
 constexpr int kBgFrame = 32;    // dim_frame_encoding
 constexpr int kBgView = 27;     // 3 + 3*2*4
-
-// inverse_sample (engine/ray_sampler.py:82-85) flipped (background.py:63-68): depth of sample k, 1 -> 0
-__device__ __forceinline__ float bg_depth(int k, float r_sphere) {
-  float t = torch_linspace(0.f, 1.f, kBgN, kBgN - 1 - k);
-  float z = 0.f * (1.0f - t) + 1.0f * t;
-  return z * (1.0f / r_sphere);
-}
 
 // Background.depth2pts_outside (background.py:102-135)
 __device__ __forceinline__ void depth2pts_outside(const float o[3], const float d[3], float depth, float R, float p4[4]) {

@@ -116,27 +116,8 @@ __global__ void __launch_bounds__(128) k_sampler_init(SamplerArgs a) {
   const int Ne = a.n_eval;
   float sumsq = 0.f;
   // z_k = near*(1-t_k) + far*t_k, t = linspace(0,1,Ne); optional stratified jitter
-  for (int k = lane; k < Ne; k += 32) {
-    float t = torch_linspace(0.f, 1.f, Ne, k);
-    float zk = a.near * (1.0f - t) + far * t;
-    float zk1 = 0.f;
-    if (k + 1 < Ne) {
-      float t1 = torch_linspace(0.f, 1.f, Ne, k + 1);
-      zk1 = a.near * (1.0f - t1) + far * t1;
-    }
-    float zout = zk;
-    if (a.jitter != nullptr) {
-      float zkm = 0.f;
-      if (k > 0) {
-        float tm = torch_linspace(0.f, 1.f, Ne, k - 1);
-        zkm = a.near * (1.0f - tm) + far * tm;
-      }
-      float lower = (k == 0) ? zk : 0.5f * (zk + zkm);
-      float upper = (k == Ne - 1) ? zk : 0.5f * (zk1 + zk);
-      zout = lower + (upper - lower) * a.jitter[(size_t)r * Ne + k];
-    }
-    a.znew[(size_t)r * Ne + k] = zout;
-  }
+  for (int k = lane; k < Ne; k += 32)
+    a.znew[(size_t)r * Ne + k] = stratified_z(a.near, far, Ne, k, a.jitter ? a.jitter + (size_t)r * Ne + k : nullptr);
   __syncwarp();
   for (int k = lane; k + 1 < Ne; k += 32) {
     float d = a.znew[(size_t)r * Ne + k + 1] - a.znew[(size_t)r * Ne + k];

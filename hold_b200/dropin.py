@@ -25,6 +25,7 @@ import torch
 
 from . import capi
 from .capi import NodePose, check, lib, ptr, stream_ptr
+from .model import sampler_rand
 
 
 def _node_of(obj):
@@ -76,7 +77,7 @@ class UniformInverseSphereSampler:
 
     def inverse_sample(self, ray_dirs, cam_loc, is_training, sdf_bounding_sphere):
         z = torch.linspace(0.0, 1.0, self.N_samples, device=ray_dirs.device).unsqueeze(0).repeat(ray_dirs.shape[0], 1)
-        assert not is_training, "training-mode jitter of the background samples is generated by the caller (hold_sampler_rand)"
+        assert not is_training, "training-mode background samples: hold_b200.train.background_forward_train(..., jitter=...)"
         return z * (1.0 / sdf_bounding_sphere)
 
 
@@ -110,14 +111,10 @@ class ErrorBoundSampler:
         z = torch.empty(R, node.S, device=ray_dirs.device)
         rnd = None
         if is_training:   # randomness is an input of the library: generated here with torch, as the reference does (:70-78,:292,:328)
-            jitter = torch.rand(R, self.N_samples_eval, device=ray_dirs.device)
-            u = torch.rand(R, self.N_samples, device=ray_dirs.device)
-            # randperm(n)[:N_extra] for every possible final buffer size n = (j + 1) * N_eval (hold_sampler_rand.extra_idx)
-            extra = torch.stack([torch.randperm((j + 1) * self.N_samples_eval, device=ray_dirs.device)[: self.N_samples_extra]
-                                 for j in range(self.max_total_iters)]).int().contiguous()
+            draw = sampler_rand(R, mine, ray_dirs.device)
             rnd = capi.SamplerRand()
-            rnd.jitter, rnd.u, rnd.extra_idx = jitter.data_ptr(), u.data_ptr(), extra.data_ptr()
-            keep += [jitter, u, extra]
+            rnd.jitter, rnd.u, rnd.extra_idx = draw["jitter"].data_ptr(), draw["u"].data_ptr(), draw["extra_idx"].data_ptr()
+            keep += list(draw.values())
         self.last_iters = torch.zeros(1, dtype=torch.int32, device=ray_dirs.device)
         check(lib().hold_sample(node.ctx.h, node.slot, R, B, ptr(cam_loc), ptr(ray_dirs), C.byref(pose),
                                 C.byref(rnd) if rnd is not None else None, ptr(z), ptr(self.last_iters), stream_ptr()))

@@ -379,6 +379,20 @@ class Node(nn.Module):
         return pose, keep, out, tfs
 
 
+def sampler_rand(R, cfg, device, generator=None):
+    """The training-mode randomness of ErrorBoundSampler.get_z_vals for R rays (the library takes it as an input,
+    hold_sampler_rand), drawn with torch as the reference draws it: stratified jitter [R, N_samples_eval] (ray_sampler.py:70-78),
+    inverse-CDF uniforms u [R, N_samples] (:292) and, for every possible final buffer size n = (j + 1) * N_samples_eval, the
+    extras permutation randperm(n)[:N_samples_extra] (:328) as one int32 row of extra_idx [max_total_iters, N_samples_extra].
+    cfg: the sampler's N_samples, N_samples_eval, N_samples_extra, max_total_iters."""
+    ne = cfg["N_samples_eval"]
+    jitter = torch.rand(R, ne, device=device, generator=generator)
+    u = torch.rand(R, cfg["N_samples"], device=device, generator=generator)
+    extra = torch.stack([torch.randperm((j + 1) * ne, device=device, generator=generator)[: cfg["N_samples_extra"]]
+                         for j in range(cfg["max_total_iters"])]).int().contiguous()
+    return dict(jitter=jitter, u=u, extra_idx=extra)
+
+
 class ErrorBoundSampler:
     """engine/ray_sampler.py:88-352 behind hold_sample; bound to a Node's ctx slot."""
 

@@ -414,58 +414,65 @@ class BgRgbFn(torch.autograd.Function):
         return (None, d_in, dW[0], dW[1], db[0], db[1])
 
 
-def _embed_n(x, n_freq):
-    out = [x]
-    for k in range(n_freq):
-        f = float(2.0 ** k)
-        out += [torch.sin(x * f), torch.cos(x * f)]
-    return torch.cat(out, -1)
+class BgIntegrateFn(torch.autograd.Function):
+    """(bg_rgb [R,3], bg_rgb_only [R,3], bg_semantics [R,4]) = bg_volume_rendering (background.py:137-165) of the 32 samples per
+    ray on hold_bg_integrate; backward on hold_bg_integrate_bwd, w.r.t. sdf [R*32], rgb [R*32,3] and fg_bg_weights [R]."""
+
+    @staticmethod
+    def forward(fctx, ctx, z, sdf, rgb, fg_bg_weights):
+        fctx.set_materialize_grads(False)
+        R = z.shape[0]
+        keep = [t.detach().float().contiguous() for t in (z, sdf, rgb, fg_bg_weights)]
+        out = [torch.empty(R, n, device=z.device) for n in (3, 3, 4)]
+        check(lib().hold_bg_integrate(ctx.h, R, *(ptr(t) for t in keep), *(ptr(t) for t in out), stream_ptr()))
+        fctx.ctx, fctx.keep = ctx, keep
+        return tuple(out)
+
+    @staticmethod
+    def backward(fctx, g_rgb, g_only, g_sem):
+        z, sdf, rgb, wfg = fctx.keep
+        gs = [None if t is None else t.float().contiguous() for t in (g_rgb, g_only, g_sem)]
+        d_sdf, d_rgb, d_w = torch.empty_like(sdf), torch.empty_like(rgb), torch.empty_like(wfg)
+        check(lib().hold_bg_integrate_bwd(fctx.ctx.h, z.shape[0], ptr(z), ptr(sdf), ptr(rgb), ptr(wfg), *(ptr(t) for t in gs),
+                                          ptr(d_sdf), ptr(d_rgb), ptr(d_w), stream_ptr()))
+        return None, None, d_sdf, d_rgb, d_w
 
 
-def depth2pts_outside(ray_o, ray_d, depth, R_s):
-    """Background.depth2pts_outside (background.py:102-135), torch (no parameters reach it)."""
-    o_dot_d = (ray_d * ray_o).sum(-1)
-    under = o_dot_d ** 2 - ((ray_o ** 2).sum(-1) - R_s ** 2)
-    d_sphere = torch.sqrt(under) - o_dot_d
-    p_sphere = ray_o + d_sphere[..., None] * ray_d
-    p_mid = ray_o - o_dot_d[..., None] * ray_d
-    pmn = torch.norm(p_mid, dim=-1)
-    axis = torch.cross(ray_o, p_sphere, dim=-1)
-    axis = axis / torch.norm(axis, dim=-1, keepdim=True)
-    ang = (torch.asin(pmn / R_s) - torch.asin(pmn * depth))[..., None]
-    pn = p_sphere * torch.cos(ang) + torch.cross(axis, p_sphere, dim=-1) * torch.sin(ang) + axis * (axis * p_sphere).sum(-1, keepdim=True) * (1.0 - torch.cos(ang))
-    pn = pn / torch.norm(pn, dim=-1, keepdim=True)
-    return torch.cat([pn, depth[..., None]], -1)
+def bg_encode(ctx, ray_dirs, cam_loc, B, jitter=None):
+    """hold_bg_encode: (bg_z_vals [R,32] as inverse_sample returns them, PE-10 point rows [R*32,84], PE-4 view rows [R*32,27]),
+    rows in the flipped sample order of the background's nets.  jitter [R,32] or None: see background_forward_train."""
+    R = ray_dirs.shape[0]
+    dev = ray_dirs.device
+    z = torch.empty(R, 32, device=dev)
+    pe_pts, pe_view = torch.empty(R * 32, 84, device=dev), torch.empty(R * 32, 27, device=dev)
+    jit = None if jitter is None else jitter.detach().float().contiguous()
+    cam, dirs = cam_loc.detach().float().contiguous(), ray_dirs.detach().float().contiguous()
+    check(lib().hold_bg_encode(ctx.h, R, B, ptr(cam), ptr(dirs), ptr(jit), ptr(z), ptr(pe_pts), 84, ptr(pe_view), 27, stream_ptr()))
+    return z, pe_pts, pe_view
 
 
-def background_forward_train(bg, fg_bg_weights, ray_dirs, cam_loc, idx, B, R_s, n_bg=32, sync=True):
-    """Background.forward in training (background.py:35-100): -> dict(bg_rgb = bg_weights * bg_rgb_only, bg_rgb_only, bg_semantics),
-    differentiable w.r.t. the background nets, its frame codes and the foreground's bg_weights.  Eval-mode (deterministic) inverse
-    sphere samples; the nets run on hold_linear (node -1), their weights must have been packed in tensor-core mode."""
+def background_forward_train(bg, fg_bg_weights, ray_dirs, cam_loc, idx, B, R_s, n_bg=32, sync=True, jitter=None):
+    """Background.forward in training (background.py:35-100): -> dict(bg_rgb = bg_weights * bg_rgb_only, bg_rgb_only, bg_semantics,
+    bg_z_vals), differentiable w.r.t. the background nets, its frame codes and the foreground's bg_weights.  The depths and point
+    encodings come from hold_bg_encode, the nets run on hold_linear (node -1; their weights must have been packed in tensor-core
+    mode), the integral on hold_bg_integrate.  jitter [R,32]: the training-mode uniforms of inverse_sample (ray_sampler.py:70-78,
+    drawn by the caller, e.g. torch.rand), or None for the 32 fixed shells.  The kernels take the bounding sphere from the
+    configured nodes, as hold_background does; R_s is the same scene_bounding_sphere and n_bg must be 32."""
+    assert n_bg == 32, "the background takes 32 samples per ray (N_samples_inverse_sphere)"
     if sync:
         bg.sync_weights()
     R = ray_dirs.shape[0]
-    dev = ray_dirs.device
-    z = torch.flip(torch.linspace(0.0, 1.0, n_bg, device=dev) * (1.0 / R_s), dims=[-1])[None].expand(R, n_bg)       # 1/R_s ... 0
-    pts = depth2pts_outside(cam_loc[:, None, :].expand(R, n_bg, 3), ray_dirs[:, None, :].expand(R, n_bg, 3), z, R_s).reshape(R * n_bg, 4)
+    z, pe_pts, pe_view = bg_encode(bg.ctx, ray_dirs, cam_loc, B, jitter)
     fc = bg.frame_latent_encoder(idx)                                                                                  # [B,32]
     fcp = fc[:, None, :].expand(B, (R // B) * n_bg, 32).reshape(R * n_bg, 32)
-    inp = torch.cat([_embed_n(pts, 10), fcp], 1)
     Ws = [getattr(bg.bg_implicit_network, f"lin{l}").weight for l in range(9)]
     bs = [getattr(bg.bg_implicit_network, f"lin{l}").bias for l in range(9)]
-    out = BgSdfFn.apply(bg.ctx, inp, *Ws, *bs)
+    out = BgSdfFn.apply(bg.ctx, torch.cat([pe_pts, fcp], 1), *Ws, *bs)
     sdf, feat = out[:, 0], out[:, 1:]
-    view = _embed_n(ray_dirs[:, None, :].expand(R, n_bg, 3).reshape(R * n_bg, 3), 4)
     rn = bg.bg_rendering_network
-    rgb = BgRgbFn.apply(bg.ctx, torch.cat([view, fcp, feat], 1), rn.lin0.weight, rn.lin1.weight, rn.lin0.bias, rn.lin1.bias).reshape(R, n_bg, 3)
-    dens = sdf.abs().reshape(R, n_bg)                                                                                  # AbsDensity (density.py:33-35)
-    dists = torch.cat([z[:, :-1] - z[:, 1:], torch.full((R, 1), 1e10, device=dev)], -1)
-    fe = dists * dens
-    w = (1 - torch.exp(-fe)) * torch.exp(-torch.cumsum(torch.cat([torch.zeros(R, 1, device=dev), fe[:, :-1]], -1), -1))
-    only = (w[:, :, None] * rgb).sum(1)
-    sem = torch.zeros(R, 4, device=dev)
-    sem[:, 0] = 1.0
-    return dict(bg_rgb=fg_bg_weights[:, None] * only, bg_rgb_only=only, bg_semantics=fg_bg_weights[:, None] * sem)
+    rgb = BgRgbFn.apply(bg.ctx, torch.cat([pe_view, fcp, feat], 1), rn.lin0.weight, rn.lin1.weight, rn.lin0.bias, rn.lin1.bias)
+    bg_rgb, only, sem = BgIntegrateFn.apply(bg.ctx, z, sdf, rgb, fg_bg_weights)
+    return dict(bg_rgb=bg_rgb, bg_rgb_only=only, bg_semantics=sem, bg_z_vals=z)
 
 
 class CompositeFn(torch.autograd.Function):
@@ -612,15 +619,19 @@ def prepare_loss_targets(out, node, B, P, canonical_pts, generator=None):
         out[f"{nid}.grad_theta"] = compute_gradient_samples(PointInSpace(global_sigma_xyz=xyz.cpu()), node, 256, v, B, 0.03, 0.20, generator)
 
 
-def forward_train(net, input, generator=None):
+def forward_train(net, input, generator=None, stratified=False):
     """HOLDNet.forward in training mode (hold/hold_net.py:53-134) -> the reference's output dict: epoch, step, fg_rgb, fg_weights-free
     composite keys (mask_prob, normal, depth, fg_semantics, bg_weights), <node>.* of every node's own volumetric_render, the loss
     targets of prepare_loss_targets, bg_z_vals, ray_dirs, cam_loc, index, and (forward) rgb, semantics, bg_rgb_only.
     Every floating-point output carries the autograd graph to the nets, beta, poses / transforms and codes.  Training-mode rules
     mirrored: pose conditioning is zeroed while current_epoch < 20 (mano_node.py:82-85); sampling runs without gradients
-    (ray_sampler.py, torch.no_grad)."""
+    (ray_sampler.py, torch.no_grad).
+    stratified=True samples as the reference's training step does, with randomness drawn from `generator`: every node's
+    ErrorBoundSampler gets its own sampler_rand draw (stratified jitter, random u, extras permutation), and the background's
+    inverse-sphere depths are jittered inside their strata (jitter [R,32] = torch.rand, ray_sampler.py:54-85; out["bg_z_vals"] are
+    those depths).  stratified=False keeps the eval-mode samples (linspace u, fixed extras, the 32 fixed shells)."""
     from . import ops
-    from .model import ErrorBoundSampler
+    from .model import ErrorBoundSampler, sampler_rand
 
     uv = input["uv"]
     B, P, _ = uv.shape
@@ -636,7 +647,8 @@ def forward_train(net, input, generator=None):
         node.sync_weights()
         pose, keep, srv, tfs = node.articulate(input)     # servers under autograd when the pose rows require grad
         with torch.no_grad():
-            z, _ = ErrorBoundSampler(node).get_z_vals(dirs, cam, pose, B)
+            rand = sampler_rand(B * P, node.sampler_cfg, dev, generator) if stratified else None
+            z, _ = ErrorBoundSampler(node).get_z_vals(dirs, cam, pose, B, rand=rand)
         S = z.shape[1]
         x = (cam[:, None, :] + z[:, :, None] * dirs[:, None, :]).reshape(B, P * S, 3)
         hand = node.kind == "hand"
@@ -656,13 +668,15 @@ def forward_train(net, input, generator=None):
     comp = composite(net.ctx, factors, [nd.class_id for nd in net.nodes.values()])
     out.update(comp)
     R_s = next(iter(net.nodes.values())).bounding_sphere
-    out["bg_z_vals"] = (torch.linspace(0.0, 1.0, 32, device=dev) * (1.0 / R_s))[None].expand(B * P, 32)
+    bg_jitter = torch.rand(B * P, 32, device=dev, generator=generator) if stratified else None
     out["ray_dirs"], out["cam_loc"], out["index"] = dirs, cam, input["idx"]
     rgb, sem = comp["fg_rgb"], comp["fg_semantics"]
     if getattr(net, "background", None) is not None:                        # hold_net.py:110-134
-        bgo = background_forward_train(net.background, comp["bg_weights"], dirs, cam, input["idx"], B, R_s)
+        bgo = background_forward_train(net.background, comp["bg_weights"], dirs, cam, input["idx"], B, R_s, jitter=bg_jitter)
         rgb, sem = rgb + bgo["bg_rgb"], sem + bgo["bg_semantics"]
-        out["bg_rgb_only"] = bgo["bg_rgb_only"]
+        out["bg_rgb_only"], out["bg_z_vals"] = bgo["bg_rgb_only"], bgo["bg_z_vals"]
+    else:                                                                   # inverse_sample runs without a background net too
+        out["bg_z_vals"] = bg_encode(net.ctx, dirs, cam, B, bg_jitter)[0]
     out["rgb"], out["semantics"] = rgb, sem
     if hasattr(net, "step_embedding"):
         net.step_embedding()                                                # hold_net.py:121-122: the BARF counter advances per training forward
@@ -727,13 +741,17 @@ class TrainStep:
     rank takes its share of the step's rays, runs sampler (no grad) -> nodes in training mode -> merge + integrate -> losses,
     back-propagates through the kernels above, then ONE all-reduce over a single flat gradient bucket (shard.allreduce_grads_,
     the only collective of the step: SURVEY §8e) and the optimiser step (Adam, hold.py:79-101).
-    The forward is `forward_train` (the reference's training-mode output dict).  Losses of this benchmark step: L1 rgb, L2 semantics
+    The forward is `forward_train` (the reference's training-mode output dict; stratified=True: its training-mode sampling, with
+    the draws from step()'s generator).  Losses of this benchmark step: L1 rgb, L2 semantics
     (loss_terms.py:14-21, :60-70) and the eikonal term (volsdf_utils.py:19-48; loss.py:83-87); the full reference loss incl. the
     kaolin-target terms (mano_cano, opacity_sparse) is `Loss` (pinned to the reference's module, tests/test_cpu_loss.py) on the
     same output dict once the canonical meshes are attached to the nodes."""
 
-    def __init__(self, net, lr=1e-4, n_eik=256, group=None, capturable=False):
-        self.net, self.group, self.n_eik = net, group, n_eik
+    def __init__(self, net, lr=1e-4, n_eik=256, group=None, capturable=False, stratified=False):
+        if capturable and stratified:
+            raise ValueError("capturing a stratified training step as a CUDA graph is not supported: use capturable=False with "
+                             "stratified=True")
+        self.net, self.group, self.n_eik, self.stratified = net, group, n_eik, stratified
         self.params = [p for p in net.parameters() if p.requires_grad]
         self.opt = torch.optim.Adam(self.params, lr=lr, capturable=capturable)
         self._graph = None
@@ -776,7 +794,7 @@ class TrainStep:
         return self._loss, self._parts
 
     def forward_loss(self, input, gt_rgb, gt_mask, generator=None):
-        out = forward_train(self.net, input, generator)
+        out = forward_train(self.net, input, generator, stratified=self.stratified)
         B = input["uv"].shape[0]
         eik = [((out[k].norm(2, dim=-1) - 1) ** 2).mean() for k in out if k.endswith("grad_theta")]
         if not eik:   # no canonical meshes attached to the nodes: the global branch (volsdf_utils.py:36-43), uniform in [-0.3, 0.3]^3

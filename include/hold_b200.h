@@ -262,6 +262,25 @@ int hold_background(hold_ctx* ctx, int R, int B, const float* cam_loc, const flo
                     const float* fg_bg_weights, float* bg_rgb, float* bg_rgb_only, float* bg_semantics,
                     float* bg_z_vals, void* stream);
 
+/* The background leg in pieces, for training (the nets run in between on hold_linear, node -1).
+ * hold_bg_encode: inverse_sample (engine/ray_sampler.py:82-85) and the per-sample inputs of Background.forward for R rays (B frames,
+ * frame-major).  jitter [R,32] (or NULL: the fixed shells, as hold_background) holds training-mode uniforms in inverse_sample's
+ * order; depth j then lies in its stratum (ray_sampler.py:70-78).  Outputs: bg_z_vals [R,32] (un-flipped, as inverse_sample
+ * returns it), and for the point p = ray * 32 + k of flipped sample k (depth 1/R_s -> 0): pe_pts row p = PE-10 of
+ * depth2pts_outside (84 columns, row stride ld_pts >= 84), pe_view row p = PE-4 of the ray direction (27 columns, ld_view >= 27).
+ * The bounding sphere is the configured nodes'.
+ * hold_bg_integrate: bg_volume_rendering over those depths: sdf [R*32] and rgb [R*32,3] of the points, fg_bg_weights [R] ->
+ * bg_rgb [R,3], bg_rgb_only [R,3], bg_semantics [R,4] (any may be NULL), as hold_background computes them.
+ * hold_bg_integrate_bwd: its reverse mode.  Upstream gradients g_* (each NULL = 0) -> d_sdf [R*32], d_rgb [R*32,3],
+ * d_fg_bg_weights [R] (overwritten). */
+int hold_bg_encode(hold_ctx* ctx, int R, int B, const float* cam_loc, const float* ray_dirs, const float* jitter, float* bg_z_vals,
+                   float* pe_pts, int ld_pts, float* pe_view, int ld_view, void* stream);
+int hold_bg_integrate(hold_ctx* ctx, int R, const float* bg_z_vals, const float* sdf, const float* rgb, const float* fg_bg_weights,
+                      float* bg_rgb, float* bg_rgb_only, float* bg_semantics, void* stream);
+int hold_bg_integrate_bwd(hold_ctx* ctx, int R, const float* bg_z_vals, const float* sdf, const float* rgb, const float* fg_bg_weights,
+                          const float* g_bg_rgb, const float* g_bg_rgb_only, const float* g_bg_semantics, float* d_sdf, float* d_rgb,
+                          float* d_fg_bg_weights, void* stream);
+
 /* Building blocks exported for tests and for callers that hold canonical points already
  * (hold_utils.query_oc, meshing): ImplicitNet.forward on canonical points (shape_net.py:84-130). */
 int hold_sdf_eval(hold_ctx* ctx, int node, int P, const float* x_c /*[P,3]*/, const float* embed_w,
