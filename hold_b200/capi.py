@@ -64,6 +64,14 @@ class SamplerRand(C.Structure):
     _fields_ = [("jitter", fp), ("u", fp), ("extra_idx", fp)]
 
 
+RASTER_MAX_K = 1024
+
+
+class RasterCfg(C.Structure):
+    _fields_ = [("faces_per_pixel", C.c_int32), ("perspective_correct", C.c_int32), ("clip_barycentric_coords", C.c_int32),
+                ("cull_backfaces", C.c_int32), ("blur_radius", C.c_float), ("sigma", C.c_float)]
+
+
 EXPORTS = {
     "hold_version": (C.c_int, []),
     "hold_last_error": (C.c_char_p, []),
@@ -86,6 +94,10 @@ EXPORTS = {
     "hold_mise_destroy": (C.c_int, [C.c_void_p]),
     "hold_mesh_sdf": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_int, fp, C.c_int, C.c_int, C.c_void_p, fp, C.c_void_p, C.c_void_p]),
     "hold_off_in_surface": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "hold_raster_silhouette": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_int, fp, C.c_int, C.c_int, C.POINTER(RasterCfg),
+                                         fp, fp, fp, fp, C.c_void_p]),
+    "hold_raster_silhouette_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_int, fp, C.c_int, C.c_int, C.POINTER(RasterCfg),
+                                             fp, fp, C.c_void_p]),
     "hold_mano_lbs_bwd": (C.c_int, [C.c_void_p, C.POINTER(ManoModel), C.c_int] + [fp] * 12 + [C.c_void_p]),
     "hold_object_tf_bwd": (C.c_int, [C.c_void_p, C.c_int, fp, fp, fp, C.c_float, fp, fp, C.c_int] + [fp] * 6 + [C.c_void_p]),
     "hold_camera_rays": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, fp, fp, fp, C.c_void_p]),

@@ -15,6 +15,7 @@
 #include "background_tc.cuh"
 #include "pose_bwd.cuh"
 #include "mesh_sdf.cuh"
+#include "raster.cuh"
 #include "mise.cuh"
 #include "mc.cuh"
 #include "warp_bwd.cuh"
@@ -387,6 +388,7 @@ int hold_ctx_check(hold_ctx* ctx, void* stream) {
   if (h & 0x100) { set_error("tensor-core pipeline wait timed out (tag %d): protocol error in k_mlp_tc", (h >> 12) & 0xF); return HOLD_E_STATE; }
   if (h & kErrRayMiss) { set_error("a ray misses the scene bounding sphere (engine/ray_sampler.py:15-18)"); return HOLD_E_RAY_MISSES_SPHERE; }
   if (h & kErrNonFinite) { set_error("non-finite value (singular transform)"); return HOLD_E_NONFINITE; }
+  if (h & kErrBadFace) { set_error("a face's vertex index is outside [0, V): the rasteriser skipped the face"); return HOLD_E_BADARG; }
   return HOLD_OK;
 }
 
@@ -889,6 +891,57 @@ int hold_off_in_surface(hold_ctx* ctx, int R, int S, const float* sdf, float thr
   if (R == 0) return HOLD_OK;
   HOLD_REQUIRE(sdf != nullptr, "NULL argument");
   k_off_in_surface<<<ceil_div(R, 128), 128, 0, (cudaStream_t)stream>>>(R, S, sdf, threshold, off_surface, in_surface);
+  HOLD_LAUNCH_CHECK(ctx);
+  return HOLD_OK;
+}
+
+// Shared by the rasteriser's forward and backward: validates the arguments and writes the face records (k_raster_setup).
+static int raster_setup(hold_ctx* ctx, int B, int V, const float* verts_ndc, int F, const int32_t* faces, int H, int W,
+                        const hold_raster_cfg* cfg, RasterArgs* a, void* stream) {
+  HOLD_REQUIRE(ctx && verts_ndc && faces && cfg, "NULL argument");
+  HOLD_REQUIRE(B >= 0 && B <= 65535 && V > 0 && F > 0 && H > 0 && W > 0 && (int64_t)ceil_div(H, kRasterTile) * ceil_div(W, kRasterTile) < (1ll << 31),
+               "bad sizes B %d V %d F %d H %d W %d", B, V, F, H, W);
+  HOLD_REQUIRE(cfg->faces_per_pixel >= 1 && cfg->faces_per_pixel <= HOLD_RASTER_MAX_K, "faces_per_pixel %d outside [1, %d]",
+               cfg->faces_per_pixel, (int)HOLD_RASTER_MAX_K);
+  HOLD_REQUIRE(cfg->sigma > 0.f && isfinite(cfg->sigma) && cfg->blur_radius >= 0.f && isfinite(cfg->blur_radius),
+               "sigma %g must be > 0 and blur_radius %g >= 0", cfg->sigma, cfg->blur_radius);
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  *a = RasterArgs{};
+  a->V = V, a->F = F, a->H = H, a->W = W, a->K = cfg->faces_per_pixel;
+  while ((1ll << a->fbits) < F) ++a->fbits;
+  a->o = raster::Opts{cfg->blur_radius, cfg->sigma, cfg->perspective_correct != 0, cfg->clip_barycentric_coords != 0,
+                      cfg->cull_backfaces != 0};
+  if (B == 0) return HOLD_OK;
+  WS(WS_RASTER, float4, (size_t)B * F * 4, rec);
+  k_raster_setup<<<dim3(ceil_div(F, 128), B), 128, 0, (cudaStream_t)stream>>>(V, F, verts_ndc, faces, a->o, rec, ctx->dev_err);
+  HOLD_LAUNCH_CHECK(ctx);
+  a->rec = rec;
+  return HOLD_OK;
+}
+
+int hold_raster_silhouette(hold_ctx* ctx, int B, int V, const float* verts_ndc, int F, const int32_t* faces, int H, int W,
+                           const hold_raster_cfg* cfg, float* sil, int64_t* pix_to_face, float* zbuf, float* dists, void* stream) {
+  HOLD_REQUIRE(sil != nullptr, "NULL argument");
+  const int nfrag = (pix_to_face != nullptr) + (zbuf != nullptr) + (dists != nullptr);
+  HOLD_REQUIRE(nfrag == 0 || nfrag == 3, "pix_to_face, zbuf and dists are given together or not at all");
+  RasterArgs a;
+  int rc = raster_setup(ctx, B, V, verts_ndc, F, faces, H, W, cfg, &a, stream);
+  if (rc || B == 0) return rc;
+  a.sil = sil, a.p2f = pix_to_face, a.zbuf = zbuf, a.dists = dists;
+  k_raster<false><<<dim3(ceil_div(H, kRasterTile) * ceil_div(W, kRasterTile), B), kRasterThreads, 0, (cudaStream_t)stream>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  return HOLD_OK;
+}
+
+int hold_raster_silhouette_bwd(hold_ctx* ctx, int B, int V, const float* verts_ndc, int F, const int32_t* faces, int H, int W,
+                               const hold_raster_cfg* cfg, const float* g_sil, float* g_verts, void* stream) {
+  HOLD_REQUIRE(g_sil != nullptr && g_verts != nullptr, "NULL argument");
+  RasterArgs a;
+  int rc = raster_setup(ctx, B, V, verts_ndc, F, faces, H, W, cfg, &a, stream);
+  if (rc || B == 0) return rc;
+  a.g_sil = g_sil, a.g_verts = g_verts;
+  HOLD_CUDA(cudaMemsetAsync(g_verts, 0, sizeof(float) * (size_t)B * V * 3, (cudaStream_t)stream));
+  k_raster<true><<<dim3(ceil_div(H, kRasterTile) * ceil_div(W, kRasterTile), B), kRasterThreads, 0, (cudaStream_t)stream>>>(a);
   HOLD_LAUNCH_CHECK(ctx);
   return HOLD_OK;
 }

@@ -24,6 +24,7 @@ constexpr int kMaxZ = 640;     // n_samples_eval * max_total_iters upper bound s
 // device error word bits
 constexpr int kErrRayMiss = 1;
 constexpr int kErrNonFinite = 2;
+constexpr int kErrBadFace = 4;   // a face's vertex index is outside [0, V) (the rasteriser skips the face)
 
 struct SamplerState {  // device-resident, one per node; written only by single-thread epilogues
   int iters;           // rounds executed so far
@@ -50,7 +51,7 @@ struct PackedNet {
 
 // grow-only workspaces of a hold_ctx, one per purpose
 enum WsSlot { WS_Z = 0, WS_SDF, WS_ZNEW, WS_SDFNEW, WS_BETA, WS_FAR, WS_XC, WS_SSDF, WS_GRAD, WS_FEAT, WS_PE, WS_ZTMP, WS_SIG,
-              WS_BGSDF, WS_BGFEAT, WS_BGRGB, WS_AMAX, WS_WARPBWD, WS_COUNT };
+              WS_BGSDF, WS_BGFEAT, WS_BGRGB, WS_AMAX, WS_WARPBWD, WS_RASTER, WS_COUNT };
 
 struct NodeState {
   bool configured = false, has_weights = false, has_rig = false;

@@ -174,6 +174,32 @@ int hold_mesh_sdf(hold_ctx* ctx, int B, int P, const float* points, int V, const
  * R rays, off_surface = min sdf > threshold, in_surface = min sdf <= 0 (uint8 flags, each output nullable). */
 int hold_off_in_surface(hold_ctx* ctx, int R, int S, const float* sdf, float threshold, uint8_t* off_surface,
                         uint8_t* in_surface, void* stream);
+/* Soft-silhouette mesh rasterisation for the pose refinement of optimize_ckpt.py (fitting/utils.py:101-118): pytorch3d
+ * v0.7.4's MeshRasterizer + SoftSilhouetteShader, restated (unpinned; the rules are in hold_b200/csrc/raster_phases.h).
+ * verts_ndc [B,V,3]: x, y in pytorch3d NDC (+x left, +y up, the shorter image side spans [-1, 1]), z = view-space depth;
+ * faces [F,3] int32, shared by the B frames, every index in [0, V) (the caller checks: the kernel skips a bad face and sets the
+ * device error word that hold_ctx_check reports as HOLD_E_BADARG).
+ *   hold_raster_silhouette: sil [B,H,W] = 1 - prod_k (1 - sigmoid(-signed_dist_k / sigma)) over the faces_per_pixel nearest
+ *   candidates of each pixel (smallest (pz, face)).  pix_to_face (int64, packed b*F + f), zbuf, dists (signed squared distance)
+ *   [B,H,W,K] are pytorch3d's fragments sorted by pz with -1 in empty slots; all three or none (NULL: nothing of size K per
+ *   pixel is written or allocated).
+ *   hold_raster_silhouette_bwd: g_sil [B,H,W] -> g_verts [B,V,3] (overwritten; x and y only: z, the selection and the culling
+ *   carry no gradient, as in pytorch3d).  Accumulated with fp32 atomics, so not bitwise reproducible; recomputes the
+ *   selection rather than storing it. */
+enum { HOLD_RASTER_MAX_K = 1024 };
+typedef struct hold_raster_cfg {
+  int32_t faces_per_pixel;         /* K, 1 .. HOLD_RASTER_MAX_K */
+  int32_t perspective_correct;     /* pytorch3d's default for perspective cameras: 1 */
+  int32_t clip_barycentric_coords; /* pytorch3d's default: blur_radius > 0 */
+  int32_t cull_backfaces;          /* default 0 */
+  float blur_radius;               /* compared with the SQUARED distance; soft silhouette: ln(1/1e-4 - 1) * sigma */
+  float sigma;                     /* BlendParams.sigma, 1e-4 */
+} hold_raster_cfg;
+int hold_raster_silhouette(hold_ctx* ctx, int B, int V, const float* verts_ndc, int F, const int32_t* faces, int H, int W,
+                           const hold_raster_cfg* cfg, float* sil, int64_t* pix_to_face, float* zbuf, float* dists, void* stream);
+int hold_raster_silhouette_bwd(hold_ctx* ctx, int B, int V, const float* verts_ndc, int F, const int32_t* faces, int H, int W,
+                               const hold_raster_cfg* cfg, const float* g_sil, float* g_verts, void* stream);
+
 /* GPU Multiresolution IsoSurface Extraction (SURVEY §8f rank 4) — the class `mise.MISE` of code/src/libmise/mise.pyx (the
  * reference's only native code) as driven by generate_mesh (utils/meshing.py:9-72): same query / update / to_dense rounds,
  * same dense (R+1)^3 value grid, R = resolution_0 << depth, bit for bit; marching cubes stays with the caller (skimage).
