@@ -1110,6 +1110,26 @@ int hold_debug_set(hold_ctx* ctx, int key, int value) {
   return HOLD_OK;
 }
 
+#ifdef HOLD_TC_PHASE_TIMING
+/* measurement build only (tools/prof_mlp_phases.py): the tensor-core MLP kernels' phase clocks since the last call, summed over
+ * the CTAs, as out[kTcMaxSteps layers][2 warpgroups][kPhSlots]; the device counters are zeroed. */
+int hold_tc_phase_read(hold_ctx* ctx, unsigned long long* out) {
+  if (!ctx || !out) return HOLD_E_BADARG;
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  HOLD_CUDA(cudaDeviceSynchronize());
+  static unsigned long long host[kPhMaxCtas][kTcMaxSteps][2][kPhSlots];
+  HOLD_CUDA(cudaMemcpyFromSymbol(host, g_tc_phase, sizeof(host)));
+  for (int i = 0; i < kTcMaxSteps * 2 * kPhSlots; ++i) {
+    out[i] = 0;
+    for (int c = 0; c < kPhMaxCtas; ++c) out[i] += (&host[c][0][0][0])[i];
+  }
+  void* dev = nullptr;
+  HOLD_CUDA(cudaGetSymbolAddress(&dev, g_tc_phase));
+  HOLD_CUDA(cudaMemset(dev, 0, sizeof(host)));
+  return HOLD_OK;
+}
+#endif
+
 /* debug/test hook (not in the public header): workspace slot pointers of the last call */
 int hold_debug_ws_copy(hold_ctx* ctx, int slot, void* dst, size_t bytes) {
   if (!ctx || slot < 0 || slot >= WS_COUNT || ctx->ws[slot].bytes < bytes) return HOLD_E_BADARG;

@@ -5,7 +5,10 @@
 //                  m64n256k16 over the layer's weight stages into a [64 x 256] fp32 accumulator held in its registers (128 per
 //                  thread), then runs the epilogue on those registers: bias + activation in fp32, split into fp16 hi/lo, and
 //                  write the next layer's A operand (SW128 K-major) for its own 64 rows back to shared memory.  The two
-//                  warpgroups share only the weight ring, so one warpgroup's epilogue overlaps the other's MMAs.
+//                  warpgroups run in lockstep: they consume the same weight ring, a stage is refilled only after all 8 consumer
+//                  warps have released it, and the ring holds 3 of a layer's 8 stages, so they drift by at most two stages
+//                  (measured: 4 .. 350 clocks of an ~18 000-clock layer).  A layer therefore costs its MMAs (at the tensor pipe's
+//                  floor, ~12 000 clocks) PLUS its epilogue; phase table in DESIGN.md §3.1 (tools/prof_mlp_phases.py).
 //   * warp 8     : (of a third warpgroup that hands its registers to the consumers through setmaxnreg) bulk-async (TMA engine) copies of pre-swizzled fp16 weight chunks L2 -> smem ring, mbarrier handshake
 //                  (full: transaction count; empty: one arrival per consumer warp once its wgmma group has read the stage).
 // Arithmetic: every fp32 operand x is split x = hi + lo (fp16 each: 11 + 11 mantissa bits) and each product is
@@ -44,6 +47,9 @@ constexpr float kTcScaleA = 64.0f, kTcScaleW = 1024.0f, kTcUnscale = 1.0f / (64.
 constexpr int kTcAccComp = 12;
 
 constexpr int kTcMaxSteps = 17;
+// Node SDF nets: lin3 has 256 - kEmbed outputs, the point's embedding re-enters at this column of layer 4's operand (api.cu
+// SkipNetShape::n_out; tc_launch_sdf refuses a net packed otherwise).
+constexpr int kTcSkipN = 256 - kEmbed;
 struct TcLayer {
   const uint8_t* wimg;  // pre-swizzled stage images, nst * 32 KB
   const float* bias;    // [256]
@@ -297,6 +303,71 @@ struct TcCfg {
   static constexpr int kSmemBytes = kSmemA + kSmemW + 256 + 1024;  // + barriers (2 x 3, 8 B each) and the abort flag + 1 KB alignment slack
 };
 
+// Phase timing of the consumer warpgroups (measurement only: -DHOLD_TC_PHASE_TIMING, tools/prof_mlp_phases.py; the shipped
+// library compiles every call below to nothing).  Lane 0 of each consumer warp adds SM-clock deltas into
+// g_tc_phase[CTA][layer][warpgroup][slot]; a slot of a (layer, warpgroup) therefore holds the sum over the warpgroup's 4 warps
+// and over the CTA's tiles, and kPhCount the number of terms.  A layer is kPhHead (layer start to the first wgmma: stage 0's wait
+// and agreement) + kPhMma (first wgmma issued to wgmma_wait<0> returning) + kPhEpilogue + kPhFence (fence.proxy.async and the
+// warpgroup barrier); kPhWaitFull and kPhStageBar are the sums over the layer's stages of the wait for a full weight stage and of
+// the warpgroup's per-stage agreement, and lie inside kPhHead (stage 0) and kPhMma (later stages).  The drift is warpgroup 0's layer-start clock minus warpgroup 1's,
+// taken from two small shared-memory tables when warpgroup 0 starts the NEXT layer (the ring lets the warpgroups drift by at most
+// two stages, so the other warpgroup has started the layer by then).
+enum { kPhWaitFull = 0, kPhStageBar, kPhHead, kPhMma, kPhEpilogue, kPhFence, kPhPrologue, kPhDrift, kPhDriftAbs, kPhCount, kPhSlots };
+#ifdef HOLD_TC_PHASE_TIMING
+constexpr int kPhMaxCtas = 160;
+__device__ unsigned long long g_tc_phase[kPhMaxCtas][kTcMaxSteps][2][kPhSlots];
+struct PhaseTimer {
+  unsigned long long* out;      // this CTA's, this warpgroup's slots of layer 0; layer stride 2 * kPhSlots
+  volatile uint32_t* starts;    // shared memory: layer-start clocks [2 warpgroups][kTcMaxSteps]
+  uint32_t t, wait, bar, t0, first;
+  int wg;
+  bool rec;
+  __device__ __forceinline__ void init(uint8_t* smem_slots, int wg_, int lane) {
+    out = &g_tc_phase[blockIdx.x][0][wg_][0], starts = reinterpret_cast<volatile uint32_t*>(smem_slots), wg = wg_;
+    rec = (lane == 0) && blockIdx.x < kPhMaxCtas;
+  }
+  __device__ __forceinline__ void add(int l, int slot, uint32_t d) {
+    if (rec) atomicAdd(out + l * 2 * kPhSlots + slot, (unsigned long long)d);
+  }
+  __device__ __forceinline__ void drift_of(int l) {   // warp 0 only
+    if (!rec || wg != 0 || (threadIdx.x >> 5) != 0) return;
+    const int d = (int)(starts[l] - starts[kTcMaxSteps + l]);
+    atomicAdd(out + l * 2 * kPhSlots + kPhDrift, (unsigned long long)(long long)d);
+    atomicAdd(out + l * 2 * kPhSlots + kPhDriftAbs, (unsigned long long)(d < 0 ? -d : d));
+  }
+  __device__ __forceinline__ void mark() { t = (uint32_t)clock(); }
+  __device__ __forceinline__ void lap(int l, int slot) { const uint32_t n = (uint32_t)clock(); add(l, slot, n - t); t = n; }
+  __device__ __forceinline__ void layer_start(int l) {
+    mark();
+    t0 = t, wait = bar = 0;
+    if (rec && (threadIdx.x & 127) == 0) starts[wg * kTcMaxSteps + l] = t;
+    if (l > 0) drift_of(l - 1);
+  }
+  __device__ __forceinline__ void stage_wait_done() { const uint32_t n = (uint32_t)clock(); wait += n - t; t = n; }
+  __device__ __forceinline__ void stage_bar_done(int s) {
+    const uint32_t n = (uint32_t)clock();
+    bar += n - t;
+    if (s == 0) first = n;   // first wgmma of the layer: start of the kPhMma span (later stages' waits lie inside it)
+  }
+  __device__ __forceinline__ void mma_done(int l) {
+    const uint32_t n = (uint32_t)clock();
+    add(l, kPhWaitFull, wait), add(l, kPhStageBar, bar), add(l, kPhHead, first - t0), add(l, kPhMma, n - first), add(l, kPhCount, 1);
+    t = n;
+  }
+};
+#else
+struct PhaseTimer {
+  __device__ __forceinline__ void init(uint8_t*, int, int) {}
+  __device__ __forceinline__ void drift_of(int) {}
+  __device__ __forceinline__ void mark() {}
+  __device__ __forceinline__ void lap(int, int) {}
+  __device__ __forceinline__ void layer_start(int) {}
+  __device__ __forceinline__ void stage_wait_done() {}
+  __device__ __forceinline__ void stage_bar_done(int) {}
+  __device__ __forceinline__ void mma_done(int) {}
+};
+#endif
+
 // Weight ring and A operand of one consumer warpgroup.
 struct Pipe {
   uint32_t a_hi, a_lo;     // this warpgroup's 64 rows of A chunk 0 (hi / lo part), shared-space addresses
@@ -304,6 +375,7 @@ struct Pipe {
   uint32_t stage, phase;
   int ns, lane, bar_id;
   volatile int* abort_flag;
+  PhaseTimer T;
 };
 
 // All MMAs of layer l for this warpgroup: acc = A . W_l^T over the layer's k stages (PASSES MMAs per k16 step).  A stage is released
@@ -314,12 +386,16 @@ template <int PASSES>
 __device__ __forceinline__ bool mma_layer_p(const TcArgs& a, Pipe& P, const int l, float (&acc)[128]) {
   const int nst = a.L[l].nst;
   uint32_t prev = 0;
+  P.T.layer_start(l);
   for (int s = 0; s < nst; ++s) {
+    P.T.mark();
     const bool got = mbar_wait(P.bWFull + 8 * P.stage, P.phase, a.err, 3, P.abort_flag);
+    P.T.stage_wait_done();
     if (!wg_all(got, P.bar_id)) {
       wgmma_wait<0>();
       return false;
     }
+    P.T.stage_bar_done(s);
     const uint32_t wb = P.sW + P.stage * kTcStageBytes;
     const int c = s >> 1;  // 64-wide A chunk holding this 32-k stage
     wgmma_fence();
@@ -344,6 +420,7 @@ __device__ __forceinline__ bool mma_layer_p(const TcArgs& a, Pipe& P, const int 
     if (++P.stage == (uint32_t)P.ns) { P.stage = 0; P.phase ^= 1; }
   }
   wgmma_wait<0>();
+  P.T.mma_done(l);
   __syncwarp();
   if (P.lane == 0) mbar_arrive(P.bWEmpty + 8 * prev);
   return true;
@@ -384,11 +461,18 @@ __device__ __forceinline__ void frag_store_a(const Frag& F, int h, int j, float 
 template <int MODE, bool HEAD, bool WRITE, bool FEAT, bool SKIP>
 __device__ __forceinline__ void epi_layer(const TcArgs& a, Frag& F, const int l, const float (&acc)[128]) {
   constexpr bool kColorLike = (MODE == MLP_COLOR || MODE == MLP_BG_RGB);
-  const int N = a.L[l].N;
+  // The unrolled loop is straight-line code, and it runs at the epilogue's pace only while it fits the instruction cache (the plain
+  // body is ~22 KB; tools/prof_mlp_phases.py, DESIGN.md §3.1).  With the skip column a run-time value every one of the 64 (j, h)
+  // instances carried its own inlined embedding: ~160 KB, 6x the clocks of a plain layer.  The node nets' skip column is the
+  // compile-time kTcSkipN, so only the one column group that mixes activation and embedding keeps that code in the loop; the groups
+  // that are embedding alone are written by the rolled loop below.  (The background net keeps its run-time N.)
+  constexpr bool kNodeSkip = SKIP && MODE != MLP_BG_SDF;
+  const int N = kNodeSkip ? kTcSkipN : a.L[l].N;
   const float* bias = a.L[l].bias;
   const float us = FEAT ? a.unscale : a.unscale * kTcScaleA;
 #pragma unroll
   for (int j = 0; j < 32; ++j) {
+    if (kNodeSkip && 8 * j >= kTcSkipN) continue;
     const int c0 = 8 * j + 2 * F.q;
     const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + c0));
     float2 w0, w1, w2;
@@ -429,6 +513,17 @@ __device__ __forceinline__ void epi_layer(const TcArgs& a, Frag& F, const int l,
       }
     }
   }
+  if (kNodeSkip) {
+#pragma unroll 1
+    for (int j = (kTcSkipN + 7) / 8; j < 32; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float ev[2];
+        const uint32_t ok = embed2<3, false>(8 * j + 2 * F.q - kTcSkipN, kEmbed, F.pt[h], a.embed_w, ev);
+        frag_store_a(F, h, j, (ok & 1u) ? kTcScaleA * ev[0] : 0.f, (ok & 2u) ? kTcScaleA * ev[1] : 0.f);
+      }
+    }
+  }
 }
 
 // Reverse-mode chain (MODE MLP_SDF_REV), one step = one accumulator: d sdf/d z_7 = w_sdf * s_7;  d sdf/d z_{l-1} = (g_l . W_l) * s_{l-1};
@@ -463,9 +558,9 @@ __device__ __forceinline__ void rev_step(const TcArgs& a, Frag& F, uint32_t* sig
         o0 = softplus100_scaled(z0, e0), o1 = softplus100_scaled(z1, e1);
         const float q0 = mufu_rcp(1.0f + e0), q1 = mufu_rcp(1.0f + e1);
         __stcg(sigw + ((l * 32 + j) * 2 + h) * kTcConsumers, unorm16_pack2((z0 >= 0.f) ? q0 : e0 * q0, (z1 >= 0.f) ? q1 : e1 * q1));
-        if (SPEC == 1 && 8 * j + 8 > 217) {
+        if (SPEC == 1 && 8 * j + 8 > kTcSkipN) {
           float ev[2];
-          const uint32_t ok = embed2<3, false>(c0 - 217, kEmbed, F.pt[h], a.embed_w, ev);
+          const uint32_t ok = embed2<3, false>(c0 - kTcSkipN, kEmbed, F.pt[h], a.embed_w, ev);
           o0 = (ok & 1u) ? kTcScaleA * ev[0] : o0;
           o1 = (ok & 2u) ? kTcScaleA * ev[1] : o1;
         }
@@ -485,8 +580,8 @@ __device__ __forceinline__ void rev_step(const TcArgs& a, Frag& F, uint32_t* sig
             const float k2 = us * (kTcScaleA * kInvQ);
             o0 = (r0 * k2) * s0, o1 = (r1 * k2) * s1;
           }
-          if ((KIND == 2 && SPEC == 1 && 8 * j + 8 > 217) || (KIND == 3 && 8 * j < 40)) {  // columns that are d sdf / d embed
-            const int e0 = (KIND == 2) ? c0 - 217 : c0;
+          if ((KIND == 2 && SPEC == 1 && 8 * j + 8 > kTcSkipN) || (KIND == 3 && 8 * j < 40)) {  // columns that are d sdf / d embed
+            const int e0 = (KIND == 2) ? c0 - kTcSkipN : c0;
             float dv[2];
             const uint32_t ok = embed2<3, true>(e0, kEmbed, F.pt[h], a.embed_w, dv);
             const float rr[2] = {r0 * us, r1 * us};
@@ -685,6 +780,7 @@ __global__ void __launch_bounds__(kTcThreadsTotal, 1) k_mlp_tc(TcArgs a) {
   P.a_hi = sA_hi + wg * 64 * 128, P.a_lo = sA_lo + wg * 64 * 128;   // 64 rows x 128 bytes of every A chunk
   P.sW = sW, P.bWFull = bWFull, P.bWEmpty = bWEmpty, P.stage = 0, P.phase = 0, P.ns = NS, P.lane = lane, P.bar_id = 1 + wg;
   P.abort_flag = abort_flag;
+  P.T.init(gen_base + (sBar - base) + 64, wg, lane);   // the barrier block's unused bytes [64, 200)
   Frag F;
   F.q = lane & 3;
   F.lo_off = (uint32_t)(NA * kTcAChunkBytes);
@@ -700,6 +796,7 @@ __global__ void __launch_bounds__(kTcThreadsTotal, 1) k_mlp_tc(TcArgs a) {
 
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     // ---------------------------------------------------------- prologue: layer-0 A operand of this warpgroup's rows
+    P.T.mark();
     prologue<MODE>(a, gA_hi, gA_lo, wg * 64 + (tid & 63), tile * kTcRows + wg * 64 + (tid & 63), tid >> 6);
     fence_proxy_async();
 #pragma unroll
@@ -722,6 +819,7 @@ __global__ void __launch_bounds__(kTcThreadsTotal, 1) k_mlp_tc(TcArgs a) {
       }
     }
     wg_all(true, P.bar_id);   // the operand is complete before any thread of the warpgroup issues the first MMA
+    P.T.lap(0, kPhPrologue);
 
     // ---------------------------------------------------------- layers: MMAs, then the epilogue on the accumulator
     bool ok = true;
@@ -763,8 +861,10 @@ __global__ void __launch_bounds__(kTcThreadsTotal, 1) k_mlp_tc(TcArgs a) {
         } else {
           rev_step<3, 0>(a, F, sigw, st, acc);
         }
+        P.T.lap(st, kPhEpilogue);
         fence_proxy_async();
         wg_all(true, P.bar_id);   // the next layer's operand is complete
+        P.T.lap(st, kPhFence);
       }
       if (!ok) break;
 #pragma unroll
@@ -787,8 +887,10 @@ __global__ void __launch_bounds__(kTcThreadsTotal, 1) k_mlp_tc(TcArgs a) {
         else if (head_layer) epi_layer<MODE, true, false, false, false>(a, F, l, acc);
         else if (!kColorLike && l == 3) epi_layer<MODE, false, true, false, true>(a, F, l, acc);
         else epi_layer<MODE, false, true, false, false>(a, F, l, acc);
+        P.T.lap(l, kPhEpilogue);
         fence_proxy_async();
         wg_all(true, P.bar_id);   // the next layer's operand is complete
+        P.T.lap(l, kPhFence);
       }
       if (!ok) break;
       // ---------------------------------------------------------- heads: sum over the 4 threads of each row
@@ -810,6 +912,7 @@ __global__ void __launch_bounds__(kTcThreadsTotal, 1) k_mlp_tc(TcArgs a) {
     }
     // every thread of the warpgroup has finished with this tile's operand before the next tile's prologue overwrites it
     wg_all(true, P.bar_id);
+    P.T.drift_of(a.n_layers - 1);
   }
 }
 
@@ -918,6 +1021,7 @@ static int tc_launch_sdf(hold_ctx* ctx, const PackedNet& net, int P, const float
   memset(&a, 0, sizeof(a));
   a.P = P, a.n_layers = rev ? 17 : 8;
   tc_layers(net, true, a);
+  HOLD_REQUIRE(net.N[3] == kTcSkipN, "node SDF net: the skip layer must have 256 - 39 outputs");
   a.xc = xc, a.embed_w = embed_w, a.sdf = sdf, a.grad = grad, a.feat = feat, a.st = st, a.err = ctx->dev_err;
   a.passes = (st != nullptr && ctx->sampler_passes >= 1 && ctx->sampler_passes <= 3) ? ctx->sampler_passes : 3;
   a.unscale = kTcUnscale * (1.0f + (float)(ctx->tc_acc_comp >= 0 ? ctx->tc_acc_comp : kTcAccComp) * (1.0f / 16777216.0f));
