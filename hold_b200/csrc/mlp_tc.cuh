@@ -443,13 +443,31 @@ struct Frag {
   float gz[2];           // reverse mode: d sdf / d z (head[h][1], head[h][2] hold d/dx, d/dy)
 };
 
-// two fp16 hi/lo pairs of the next layer's operand for accumulator columns c0 = 8 j + 2 q, c0 + 1 of row h
+// two fp16 hi/lo pairs of the next layer's operand for accumulator columns c0 = 8 j + 2 q, c0 + 1 of row h (row: F.a_row[h], or that
+// plus a whole number of A chunks)
+__device__ __forceinline__ void store_a_pair(uint8_t* row, int r7, uint32_t lo_off, int j, float o0, float o1) {
+  uint32_t hi, lo;
+  split2(o0, o1, hi, lo);
+  uint8_t* dst = row + (j >> 3) * kTcAChunkBytes + (((j & 7) ^ r7) << 4);
+  *reinterpret_cast<uint32_t*>(dst) = hi;
+  *reinterpret_cast<uint32_t*>(dst + lo_off) = lo;
+}
 __device__ __forceinline__ void frag_store_a(const Frag& F, int h, int j, float o0, float o1) {
+  store_a_pair(F.a_row[h], F.r7[h], F.lo_off, j, o0, o1);
+}
+// the same for the columns of the pair selected by `mask` (bit i: column c0 + i) only
+__device__ __forceinline__ void frag_store_a_cols(const Frag& F, int h, int j, uint32_t mask, float o0, float o1) {
   uint32_t hi, lo;
   split2(o0, o1, hi, lo);
   uint8_t* dst = F.a_row[h] + (j >> 3) * kTcAChunkBytes + (((j & 7) ^ F.r7[h]) << 4);
-  *reinterpret_cast<uint32_t*>(dst) = hi;
-  *reinterpret_cast<uint32_t*>(dst + F.lo_off) = lo;
+  if (mask == 3u) {
+    *reinterpret_cast<uint32_t*>(dst) = hi;
+    *reinterpret_cast<uint32_t*>(dst + F.lo_off) = lo;
+  } else if (mask != 0u) {
+    const int i = (int)(mask >> 1);
+    *reinterpret_cast<uint16_t*>(dst + 2 * i) = (uint16_t)(hi >> (16 * i));
+    *reinterpret_cast<uint16_t*>(dst + F.lo_off + 2 * i) = (uint16_t)(lo >> (16 * i));
+  }
 }
 
 // One layer of a forward chain (every mode but the reverse-mode gradient and hold_linear), on the accumulator in registers:
@@ -526,79 +544,124 @@ __device__ __forceinline__ void epi_layer(const TcArgs& a, Frag& F, const int l,
   }
 }
 
-// Reverse-mode chain (MODE MLP_SDF_REV), one step = one accumulator: d sdf/d z_7 = w_sdf * s_7;  d sdf/d z_{l-1} = (g_l . W_l) * s_{l-1};
-// the embedding columns (skip input of layer 4, input of layer 0) collect d sdf/d embed, chained with d embed/d x_c per column.
-//   KIND 0: forward layer l = st (stashes s_l = softplus'(z_l));  SPEC 1: l = 3 (skip columns), SPEC 2: l = 7 (sdf head)
+// Reverse-mode chain (MODE MLP_SDF_REV): d sdf/d z_7 = w_sdf * s_7;  d sdf/d z_{l-1} = (g_l . W_l) * s_{l-1};  the embedding columns
+// (skip input of layer 4, input of layer 0) collect d sdf/d embed, chained with d embed/d x_c per column (rev_embed_chain).
+// The epilogues are straight-line code and hold their pace only while a body fits the instruction cache (~22 KB, DESIGN.md §3.1),
+// so there is ONE body per layer kind, inlined at one call site of the kernel's (rolled) layer loop, which stays warm from one
+// layer to the next; the columns that differ between layers of a kind are handled outside it by small rolled loops.  A body walks
+// the accumulator in two passes of 16 column groups through one unrolled copy, each element chosen from acc[k] or acc[64 + k] by a
+// warp-uniform select.  The epilogue never writes the accumulator: a copy between its registers would leave two wgmma operands
+// holding one value, and ptxas would then insert moves between the next layer's wgmmas and serialise them.
+//   KIND 0: forward layer l = st (stashes s_l = softplus'(z_l)); the sdf head of layer 7 is in the body with weights times 0 elsewhere
 //   KIND 1: the feature layer (st = 8): writes the 256-d feature, seeds g_7 = w_sdf * s_7
-//   KIND 2: backward layer l = 16 - st: operand of the next step = acc * s_{l-1};  SPEC 1: l = 4 (its columns >= 217 are d sdf/d embed)
-//   KIND 3: st = 16: d sdf / d embed through layer 0's input, no operand
+//   KIND 2: backward layer l = 16 - st (st = 9..15): operand of the next step = acc * s_{l-1}
 // Stash: s_l as unorm16 pairs, written and later read by the SAME thread (its fragment), L2 only (.cg), laid out so that a warp's
 // 32 words of one (layer, column pair, row half) are contiguous: 512 KB per CTA.
-template <int KIND, int SPEC>
-__device__ __forceinline__ void rev_step(const TcArgs& a, Frag& F, uint32_t* sigw, const int st, const float (&acc)[128]) {
+template <int KIND>
+__device__ __forceinline__ void rev_layer(const TcArgs& a, Frag& F, uint32_t* sigw, const int st, const float (&acc)[128]) {
   constexpr float kInvQ = 1.0f / 65535.0f;
   const int l = (st <= 8) ? st : 16 - st;
   const float* bias = (KIND <= 1) ? a.L[st].bias : nullptr;
   // stash layer read by this step: s_7 for the feature layer's seed, s_{l-1} for backward layer l
   const int sl = (KIND == 1) ? 7 : l - 1;
   const float us = (KIND == 0) ? a.unscale * kTcScaleA : a.unscale;   // forward layers work on kTcScaleA * z (bias pre-scaled)
+  const float head_w = (st == 7) ? 1.f : 0.f;                          // exact: the head's weights, or zeros
+#pragma unroll 1
+  for (int pass = 0; pass < 2; ++pass) {
+    // this pass's column groups j = 16 pass + jj (columns from 128 pass on, the A operand's chunks 2 pass, 2 pass + 1): base
+    // pointers per pass, so that every access inside the unrolled loop is the base plus an immediate
+    const int cb = 128 * pass + 2 * F.q;
+    uint8_t* const row[2] = {F.a_row[0] + 2 * pass * kTcAChunkBytes, F.a_row[1] + 2 * pass * kTcAChunkBytes};
+    uint32_t* const sp = sigw + (size_t)(((KIND == 0 ? l : sl) * 32 + 16 * pass) * 2 * kTcConsumers);
+    float* const fp[2] = {a.feat + (size_t)F.p[0] * kFeat + cb, a.feat + (size_t)F.p[1] * kFeat + cb};
 #pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    const int c0 = 8 * j + 2 * F.q;
-    float2 bv = make_float2(0.f, 0.f), wl = make_float2(0.f, 0.f);
-    if (KIND <= 1) bv = __ldg(reinterpret_cast<const float2*>(bias + c0));
-    if ((KIND == 0 && SPEC == 2) || KIND == 1) wl = __ldg(reinterpret_cast<const float2*>(a.w_last + c0));
+    for (int jj = 0; jj < 16; ++jj) {
+      float2 bv = make_float2(0.f, 0.f), wl = make_float2(0.f, 0.f);
+      if (KIND <= 1) {
+        bv = __ldg(reinterpret_cast<const float2*>(bias + cb + 8 * jj));
+        wl = __ldg(reinterpret_cast<const float2*>(a.w_last + cb + 8 * jj));
+      }
+      if (KIND == 0) wl.x *= head_w, wl.y *= head_w;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const float r0 = acc[4 * j + 2 * h], r1 = acc[4 * j + 2 * h + 1];
-      float o0 = 0.f, o1 = 0.f;
-      if (KIND == 0) {
-        float e0, e1;
-        const float z0 = fmaf(r0, us, bv.x), z1 = fmaf(r1, us, bv.y);
-        o0 = softplus100_scaled(z0, e0), o1 = softplus100_scaled(z1, e1);
-        const float q0 = mufu_rcp(1.0f + e0), q1 = mufu_rcp(1.0f + e1);
-        __stcg(sigw + ((l * 32 + j) * 2 + h) * kTcConsumers, unorm16_pack2((z0 >= 0.f) ? q0 : e0 * q0, (z1 >= 0.f) ? q1 : e1 * q1));
-        if (SPEC == 1 && 8 * j + 8 > kTcSkipN) {
-          float ev[2];
-          const uint32_t ok = embed2<3, false>(c0 - kTcSkipN, kEmbed, F.pt[h], a.embed_w, ev);
-          o0 = (ok & 1u) ? kTcScaleA * ev[0] : o0;
-          o1 = (ok & 2u) ? kTcScaleA * ev[1] : o1;
-        }
-        if (SPEC == 2) F.head[h][0] += o0 * wl.x + o1 * wl.y;
-      } else {
-        // softplus' of these 2 columns (times 65535; the scale is folded below)
-        const uint32_t sq = (KIND == 3) ? 0u : __ldcg(sigw + ((sl * 32 + j) * 2 + h) * kTcConsumers);
-        const float s0 = unorm16_lo(sq), s1 = unorm16_hi(sq);
-        if (KIND == 1) {
-          if (F.valid[h]) {   // the 256-d feature vector: written once, read once by the colour net -> streaming stores
-            __stcs(reinterpret_cast<float2*>(a.feat + (size_t)F.p[h] * kFeat + c0), make_float2(fmaf(r0, us, bv.x), fmaf(r1, us, bv.y)));
-          }
-          // g_7 = w_sdf * s_7, times the operand scale
-          o0 = (kTcScaleA * kInvQ) * wl.x * s0, o1 = (kTcScaleA * kInvQ) * wl.y * s1;
+      for (int h = 0; h < 2; ++h) {
+        const int k = 4 * jj + 2 * h;
+        const float r0 = pass ? acc[64 + k] : acc[k], r1 = pass ? acc[64 + k + 1] : acc[k + 1];
+        float o0, o1;
+        if (KIND == 0) {
+          float e0, e1;
+          const float z0 = fmaf(r0, us, bv.x), z1 = fmaf(r1, us, bv.y);
+          o0 = softplus100_scaled(z0, e0), o1 = softplus100_scaled(z1, e1);
+          const float q0 = mufu_rcp(1.0f + e0), q1 = mufu_rcp(1.0f + e1);
+          __stcg(sp + (2 * jj + h) * kTcConsumers, unorm16_pack2((z0 >= 0.f) ? q0 : e0 * q0, (z1 >= 0.f) ? q1 : e1 * q1));
+          F.head[h][0] += o0 * wl.x + o1 * wl.y;
         } else {
-          if (KIND == 2) {   // operand of the next backward layer: (acc * unscale) * s_{l-1}, times the operand scale (one constant)
+          // softplus' of these 2 columns (times 65535; the scale is folded below)
+          const uint32_t sq = __ldcg(sp + (2 * jj + h) * kTcConsumers);
+          const float s0 = unorm16_lo(sq), s1 = unorm16_hi(sq);
+          if (KIND == 1) {
+            if (F.valid[h]) {   // the 256-d feature vector: written once, read once by the colour net -> streaming stores
+              __stcs(reinterpret_cast<float2*>(fp[h] + 8 * jj), make_float2(fmaf(r0, us, bv.x), fmaf(r1, us, bv.y)));
+            }
+            // g_7 = w_sdf * s_7, times the operand scale
+            o0 = (kTcScaleA * kInvQ) * wl.x * s0, o1 = (kTcScaleA * kInvQ) * wl.y * s1;
+          } else {   // operand of the next backward layer: (acc * unscale) * s_{l-1}, times the operand scale (one constant)
             const float k2 = us * (kTcScaleA * kInvQ);
             o0 = (r0 * k2) * s0, o1 = (r1 * k2) * s1;
           }
-          if ((KIND == 2 && SPEC == 1 && 8 * j + 8 > kTcSkipN) || (KIND == 3 && 8 * j < 40)) {  // columns that are d sdf / d embed
-            const int e0 = (KIND == 2) ? c0 - kTcSkipN : c0;
-            float dv[2];
-            const uint32_t ok = embed2<3, true>(e0, kEmbed, F.pt[h], a.embed_w, dv);
-            const float rr[2] = {r0 * us, r1 * us};
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              const int ec = max(e0 + i, 0), d = ec - 3 * ((ec * 171) >> 9);
-              const bool okc = (ok >> i) & 1u;
-              const float je = okc ? rr[i] * dv[i] : 0.f;
-              F.head[h][1] += (d == 0) ? je : 0.f;
-              F.head[h][2] += (d == 1) ? je : 0.f;
-              F.gz[h] += (d == 2) ? je : 0.f;
-              if (KIND == 2 && okc) (i == 0 ? o0 : o1) = 0.f;
-            }
-          }
         }
+        store_a_pair(row[h], F.r7[h], F.lo_off, jj, o0, o1);
       }
-      if (KIND != 3) frag_store_a(F, h, j, o0, o1);
+    }
+  }
+}
+
+// Skip layer (l = 3): the operand columns >= kTcSkipN are the point's embedding (shape_net.py:116-119), written over the
+// activations the forward body stored there (whose softplus' it stashed; layer 4's backward step zeroes those columns).
+__device__ __forceinline__ void rev_skip_embed(const TcArgs& a, const Frag& F) {
+#pragma unroll 1
+  for (int j = kTcSkipN / 8; j < 32; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float ev[2];
+      const uint32_t ok = embed2<3, false>(8 * j + 2 * F.q - kTcSkipN, kEmbed, F.pt[h], a.embed_w, ev);
+      frag_store_a_cols(F, h, j, ok, kTcScaleA * ev[0], kTcScaleA * ev[1]);
+    }
+  }
+}
+
+// d sdf / d x_c through the 39 embedding columns e_col .. e_col + 38 of a backward step's accumulator (d sdf / d embed: layer 0's
+// input, e_col = 0, or layer 4's skip input, e_col = kTcSkipN) times d embed / d x_c, added per coordinate to F.head[h][1],
+// F.head[h][2], F.gz[h] in ascending columns.  The rolled loop walks the 5 column groups from j0 = e_col / 8 on and picks each
+// group's 4 accumulator values by selects, so the accumulator stays in registers.  Layer 4 (e_col = kTcSkipN) also sets the step's
+// operand columns that are embedding to 0: they are no output of layer 3.
+__device__ __forceinline__ void rev_embed_chain(const TcArgs& a, Frag& F, const bool layer4, const float (&acc)[128]) {
+  const float us = a.unscale;
+  const int e_col = layer4 ? kTcSkipN : 0, j0 = e_col / 8;
+#pragma unroll 1
+  for (int g = 0; g < 5; ++g) {
+    const int j = j0 + g, e0 = 8 * j + 2 * F.q - e_col;
+    float v[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      v[k] = 0.f;
+#pragma unroll
+      for (int gg = 0; gg < 5; ++gg) v[k] = (g == gg) ? (layer4 ? acc[4 * (kTcSkipN / 8 + gg) + k] : acc[4 * gg + k]) : v[k];
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float dv[2];
+      const uint32_t ok = embed2<3, true>(e0, kEmbed, F.pt[h], a.embed_w, dv);
+      const float rr[2] = {v[2 * h] * us, v[2 * h + 1] * us};
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int ec = max(e0 + i, 0), d = ec - 3 * ((ec * 171) >> 9);
+        const bool okc = (ok >> i) & 1u;
+        const float je = okc ? rr[i] * dv[i] : 0.f;
+        F.head[h][1] += (d == 0) ? je : 0.f;
+        F.head[h][2] += (d == 1) ? je : 0.f;
+        F.gz[h] += (d == 2) ? je : 0.f;
+      }
+      if (layer4) frag_store_a_cols(F, h, j, ok, 0.f, 0.f);
     }
   }
 }
@@ -845,21 +908,19 @@ __global__ void __launch_bounds__(kTcThreadsTotal, 1) k_mlp_tc(TcArgs a) {
         }
       }
     } else if (MODE == MLP_SDF_REV) {
-      // ======== reverse-mode gradient: 8 forward layers (stash softplus'), feature layer, 8 backward layers (rev_step) ========
+      // ======== reverse-mode gradient: 8 forward layers (stash softplus'), feature layer, 8 backward layers (rev_layer) ========
+#pragma unroll 1
       for (int st = 0; st < 17; ++st) {
         ok = mma_layer(a, P, st, acc);
         if (!ok) break;
         if (st < 8) {
-          if (st == 3) rev_step<0, 1>(a, F, sigw, st, acc);
-          else if (st == 7) rev_step<0, 2>(a, F, sigw, st, acc);
-          else rev_step<0, 0>(a, F, sigw, st, acc);
+          rev_layer<0>(a, F, sigw, st, acc);
+          if (st == 3) rev_skip_embed(a, F);
         } else if (st == 8) {
-          rev_step<1, 0>(a, F, sigw, st, acc);
-        } else if (st < 16) {
-          if (st == 12) rev_step<2, 1>(a, F, sigw, st, acc);
-          else rev_step<2, 0>(a, F, sigw, st, acc);
+          rev_layer<1>(a, F, sigw, st, acc);
         } else {
-          rev_step<3, 0>(a, F, sigw, st, acc);
+          if (st < 16) rev_layer<2>(a, F, sigw, st, acc);   // layer 0's step (st = 16) writes no operand
+          if (st == 12 || st == 16) rev_embed_chain(a, F, st == 12, acc);
         }
         P.T.lap(st, kPhEpilogue);
         fence_proxy_async();
