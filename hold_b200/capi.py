@@ -72,6 +72,14 @@ class RasterCfg(C.Structure):
                 ("cull_backfaces", C.c_int32), ("blur_radius", C.c_float), ("sigma", C.c_float)]
 
 
+KNN_MAX_K = 32
+
+
+class IcpCfg(C.Structure):
+    _fields_ = [("max_correspondence_distance", C.c_double), ("relative_fitness", C.c_double), ("relative_rmse", C.c_double),
+                ("max_iteration", C.c_int32), ("with_scaling", C.c_int32)]
+
+
 EXPORTS = {
     "hold_version": (C.c_int, []),
     "hold_last_error": (C.c_char_p, []),
@@ -98,6 +106,8 @@ EXPORTS = {
                                          fp, fp, fp, fp, C.c_void_p]),
     "hold_raster_silhouette_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_int, fp, C.c_int, C.c_int, C.POINTER(RasterCfg),
                                              fp, fp, C.c_void_p]),
+    "hold_knn_points": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, C.c_int, fp, fp, C.c_int, fp, fp, C.c_void_p]),
+    "hold_icp": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, C.c_int, fp, fp, fp, C.POINTER(IcpCfg), fp, fp, fp, fp, C.c_void_p]),
     "hold_mano_lbs_bwd": (C.c_int, [C.c_void_p, C.POINTER(ManoModel), C.c_int] + [fp] * 12 + [C.c_void_p]),
     "hold_object_tf_bwd": (C.c_int, [C.c_void_p, C.c_int, fp, fp, fp, C.c_float, fp, fp, C.c_int] + [fp] * 6 + [C.c_void_p]),
     "hold_camera_rays": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, fp, fp, fp, C.c_void_p]),

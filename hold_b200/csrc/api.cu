@@ -16,6 +16,7 @@
 #include "pose_bwd.cuh"
 #include "mesh_sdf.cuh"
 #include "raster.cuh"
+#include "pointcloud.cuh"
 #include "mise.cuh"
 #include "mc.cuh"
 #include "warp_bwd.cuh"
@@ -389,6 +390,7 @@ int hold_ctx_check(hold_ctx* ctx, void* stream) {
   if (h & kErrRayMiss) { set_error("a ray misses the scene bounding sphere (engine/ray_sampler.py:15-18)"); return HOLD_E_RAY_MISSES_SPHERE; }
   if (h & kErrNonFinite) { set_error("non-finite value (singular transform)"); return HOLD_E_NONFINITE; }
   if (h & kErrBadFace) { set_error("a face's vertex index is outside [0, V): the rasteriser skipped the face"); return HOLD_E_BADARG; }
+  if (h & kErrBadLength) { set_error("a point-cloud length is outside [0, P]: the kernel clamped it"); return HOLD_E_BADARG; }
   return HOLD_OK;
 }
 
@@ -942,6 +944,78 @@ int hold_raster_silhouette_bwd(hold_ctx* ctx, int B, int V, const float* verts_n
   a.g_sil = g_sil, a.g_verts = g_verts;
   HOLD_CUDA(cudaMemsetAsync(g_verts, 0, sizeof(float) * (size_t)B * V * 3, (cudaStream_t)stream));
   k_raster<true><<<dim3(ceil_div(H, kRasterTile) * ceil_div(W, kRasterTile), B), kRasterThreads, 0, (cudaStream_t)stream>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  return HOLD_OK;
+}
+
+int hold_knn_points(hold_ctx* ctx, int N, int P1, const float* p1, const int32_t* lengths1, int P2, const float* p2,
+                    const int32_t* lengths2, int K, float* dists, int32_t* idx, void* stream) {
+  HOLD_REQUIRE(ctx != nullptr, "ctx is NULL");
+  HOLD_REQUIRE(N >= 0 && P1 >= 0 && P2 >= 0, "bad sizes N %d P1 %d P2 %d", N, P1, P2);
+  HOLD_REQUIRE(K >= 1 && K <= HOLD_KNN_MAX_K, "K %d outside [1, %d]", K, (int)HOLD_KNN_MAX_K);
+  if (N == 0 || P1 == 0) return HOLD_OK;
+  HOLD_REQUIRE(p1 && dists && idx && (P2 == 0 || p2), "NULL argument");
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  const dim3 grid(ceil_div(P1, kPcThreads), min(N, 65535));
+  cudaStream_t s = (cudaStream_t)stream;
+#define HOLD_KNN_CASE(KT)                                                                                                    \
+  k_knn<KT><<<grid, kPcThreads, 0, s>>>(N, P1, p1, lengths1, P2, p2, lengths2, K, dists, idx, ctx->dev_err)
+  if (K == 1) HOLD_KNN_CASE(1);
+  else if (K <= 2) HOLD_KNN_CASE(2);
+  else if (K <= 4) HOLD_KNN_CASE(4);
+  else if (K <= 8) HOLD_KNN_CASE(8);
+  else if (K <= 16) HOLD_KNN_CASE(16);
+  else HOLD_KNN_CASE(32);
+#undef HOLD_KNN_CASE
+  HOLD_LAUNCH_CHECK(ctx);
+  return HOLD_OK;
+}
+
+int hold_icp(hold_ctx* ctx, int N, int Ps, const float* source, const int32_t* src_lengths, int Pt, const float* target,
+             const int32_t* tgt_lengths, const double* init, const hold_icp_cfg* cfg, double* transformation, double* fitness,
+             double* inlier_rmse, int32_t* iterations, void* stream) {
+  HOLD_REQUIRE(ctx != nullptr && cfg != nullptr, "NULL argument");
+  HOLD_REQUIRE(N >= 0 && N <= 65535 && Ps >= 0 && Pt >= 0, "bad sizes N %d Ps %d Pt %d", N, Ps, Pt);
+  HOLD_REQUIRE(cfg->max_iteration >= 0, "max_iteration %d < 0", cfg->max_iteration);
+  HOLD_REQUIRE(!isnan(cfg->max_correspondence_distance) && !isnan(cfg->relative_fitness) && !isnan(cfg->relative_rmse),
+               "NaN in hold_icp_cfg");
+  if (N == 0) return HOLD_OK;
+  HOLD_REQUIRE(transformation && fitness && inlier_rmse && iterations && (Ps == 0 || source) && (Pt == 0 || target),
+               "NULL argument");
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  IcpArgs a{};
+  a.N = N, a.Ps = Ps, a.Pt = Pt, a.nb = max(1, ceil_div(Ps, kPcThreads));
+  a.src = source, a.src_len = src_lengths, a.tgt = target, a.tgt_len = tgt_lengths, a.init = init;
+  const double md = cfg->max_correspondence_distance;
+  a.max_d2 = md > 0.0 ? md * md : -1.0;   // open3d: no correspondence unless max_correspondence_distance > 0
+  a.rel_fitness = cfg->relative_fitness, a.rel_rmse = cfg->relative_rmse, a.with_scaling = cfg->with_scaling;
+  a.err = ctx->dev_err;
+  // one workspace: pair states, transformed source, per-CTA partials, correspondences
+  const size_t b_st = (sizeof(IcpPair) * (size_t)N + 255) & ~(size_t)255;
+  const size_t b_xs = (size_t)N * Ps * 3 * sizeof(double), b_part = (size_t)N * a.nb * kIcpPart * sizeof(double);
+  const size_t o_xs = b_st, o_part = o_xs + ((b_xs + 255) & ~(size_t)255), o_corr = o_part + ((b_part + 255) & ~(size_t)255);
+  WS(WS_ICP, uint8_t, o_corr + (size_t)N * Ps * sizeof(int) + 256, ws);
+  a.st = (IcpPair*)ws, a.xs = (double*)(ws + o_xs), a.part = (double*)(ws + o_part), a.corr = (int*)(ws + o_corr);
+  cudaStream_t s = (cudaStream_t)stream;
+  const dim3 grid(a.nb, N);
+  const int pair_blocks = ceil_div(N, 128);
+  k_icp_start<<<grid, kPcThreads, 0, s>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_icp_corr<false><<<grid, kPcThreads, 0, s>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_icp_eval<<<pair_blocks, 128, 0, s>>>(a, -1);
+  HOLD_LAUNCH_CHECK(ctx);
+  for (int it = 0; it < cfg->max_iteration; ++it) {
+    k_icp_cov<<<grid, kPcThreads, 0, s>>>(a);
+    HOLD_LAUNCH_CHECK(ctx);
+    k_icp_update<<<pair_blocks, 128, 0, s>>>(a);
+    HOLD_LAUNCH_CHECK(ctx);
+    k_icp_corr<true><<<grid, kPcThreads, 0, s>>>(a);
+    HOLD_LAUNCH_CHECK(ctx);
+    k_icp_eval<<<pair_blocks, 128, 0, s>>>(a, it);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  k_icp_out<<<pair_blocks, 128, 0, s>>>(a, transformation, fitness, inlier_rmse, iterations);
   HOLD_LAUNCH_CHECK(ctx);
   return HOLD_OK;
 }

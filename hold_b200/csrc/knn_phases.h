@@ -22,19 +22,27 @@
 #if defined(__CUDA_ARCH__)
 #define HOLD_FADD(a, b) __fadd_rn((a), (b))
 #define HOLD_FMUL(a, b) __fmul_rn((a), (b))
+#define HOLD_DADD(a, b) __dadd_rn((a), (b))
+#define HOLD_DMUL(a, b) __dmul_rn((a), (b))
 #else
 #define HOLD_FADD(a, b) ((a) + (b))   // host build uses -ffp-contract=off
 #define HOLD_FMUL(a, b) ((a) * (b))
+#define HOLD_DADD(a, b) ((a) + (b))
+#define HOLD_DMUL(a, b) ((a) * (b))
 #endif
 
 namespace hold {
 namespace knnc {
 
 constexpr int kK = 15, kNV = 778, kCand = 48, kClSize = 16, kNCl = (kNV + kClSize - 1) / kClSize;   // 49 groups
-struct Top {
-  float d[kK];
-  int i[kK];
+// the K best (distance, index) pairs in lexicographic order; the MANO KNN uses TopK<15, float>, the point-cloud KNN
+// (pointcloud_phases.h) K = 1 .. 32 in float and K = 1 in double
+template <int K, typename T>
+struct TopK {
+  T d[K];
+  int i[K];
 };
+using Top = TopK<kK, float>;
 struct V4 { float x, y, z; int idx; };      // cluster-ordered vertex: position + ORIGINAL index (padding: idx < 0, far away)
 struct Cl { float x, y, z, r; };            // centre, radius
 
@@ -43,16 +51,22 @@ HOLD_HD float exact_dist(float vx, float vy, float vz, float px, float py, float
   const float dx = px - vx, dy = py - vy, dz = pz - vz;
   return HOLD_FADD(HOLD_FADD(HOLD_FMUL(dx, dx), HOLD_FMUL(dy, dy)), HOLD_FMUL(dz, dz));
 }
-HOLD_HD void insert(Top& r, float dist, int v) {   // replace the last entry, bubble up; order (distance, index)
-  r.d[kK - 1] = dist;
-  r.i[kK - 1] = v;
+// the same expression in double (the ICP correspondence search)
+HOLD_HD double exact_dist(double vx, double vy, double vz, double px, double py, double pz) {
+  const double dx = px - vx, dy = py - vy, dz = pz - vz;
+  return HOLD_DADD(HOLD_DADD(HOLD_DMUL(dx, dx), HOLD_DMUL(dy, dy)), HOLD_DMUL(dz, dz));
+}
+template <int K, typename T>
+HOLD_HD void insert(TopK<K, T>& r, T dist, int v) {   // replace the last entry, bubble up; order (distance, index)
+  r.d[K - 1] = dist;
+  r.i[K - 1] = v;
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
-  for (int k = kK - 1; k > 0; --k) {
+  for (int k = K - 1; k > 0; --k) {
     const bool sw = (r.d[k] < r.d[k - 1]) || (r.d[k] == r.d[k - 1] && r.i[k] < r.i[k - 1]);
     if (sw) {
-      const float td = r.d[k]; r.d[k] = r.d[k - 1]; r.d[k - 1] = td;
+      const T td = r.d[k]; r.d[k] = r.d[k - 1]; r.d[k - 1] = td;
       const int ti = r.i[k]; r.i[k] = r.i[k - 1]; r.i[k - 1] = ti;
     }
   }

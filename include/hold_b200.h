@@ -200,6 +200,35 @@ int hold_raster_silhouette(hold_ctx* ctx, int B, int V, const float* verts_ndc, 
 int hold_raster_silhouette_bwd(hold_ctx* ctx, int B, int V, const float* verts_ndc, int F, const int32_t* faces, int H, int W,
                                const hold_raster_cfg* cfg, const float* g_sil, float* g_verts, void* stream);
 
+/* Point-cloud evaluation (utils/eval_modules.py: pytorch3d's chamfer_distance, open3d's ICP), restated (unpinned; the rules
+ * are in hold_b200/csrc/pointcloud_phases.h).  Brute force: no [P1,P2] buffer.  A length outside [0, P] is clamped by the
+ * kernel and sets the device error word that hold_ctx_check reports as HOLD_E_BADARG; lengths NULL = all P points.
+ *   hold_knn_points: pytorch3d v0.7.4 knn_points for D = 3.  p1 [N,P1,3], p2 [N,P2,3] -> dists [N,P1,K] squared distances
+ *   ((dx*dx + dy*dy) + dz*dz in fp32, no FMA), ascending, ties to the lower index; idx [N,P1,K] int32.  Padding slots (row >=
+ *   lengths1[n] or k >= lengths2[n]) hold 0 in both.  K in [1, HOLD_KNN_MAX_K], N, P1, P2 >= 0, else HOLD_E_BADARG. */
+enum { HOLD_KNN_MAX_K = 32 };
+int hold_knn_points(hold_ctx* ctx, int N, int P1, const float* p1, const int32_t* lengths1, int P2, const float* p2,
+                    const int32_t* lengths2, int K, float* dists, int32_t* idx, void* stream);
+/*   hold_icp: open3d registration_icp with TransformationEstimationPointToPoint(with_scaling) for N independent pairs
+ *   (source [N,Ps,3], target [N,Pt,3] fp32, held in double).  The source moves by init ([N,4,4] double, NULL = identity), then by
+ *   each update; transformation = update * transformation.  A source point's correspondence is its nearest target point
+ *   (double, ties to the lower index) when d^2 < max_correspondence_distance^2.  One iteration: Umeyama update from the
+ *   correspondences, apply it, new correspondences, stop once |d fitness| < relative_fitness and |d rmse| < relative_rmse.
+ *   Outputs: transformation [N,4,4], fitness [N] (correspondences / source points), inlier_rmse [N] (0 without correspondences)
+ *   double, iterations [N] int32.  All max_iteration iterations are enqueued (a converged pair skips them on the device): no
+ *   host synchronisation, CUDA-graph capturable; fixed-order reductions, so bitwise reproducible and independent of the
+ *   other pairs of the batch. */
+typedef struct hold_icp_cfg {
+  double max_correspondence_distance;
+  double relative_fitness; /* open3d's default 1e-6 */
+  double relative_rmse;    /* 1e-6 */
+  int32_t max_iteration;   /* 30 */
+  int32_t with_scaling;    /* 0 */
+} hold_icp_cfg;
+int hold_icp(hold_ctx* ctx, int N, int Ps, const float* source, const int32_t* src_lengths, int Pt, const float* target,
+             const int32_t* tgt_lengths, const double* init, const hold_icp_cfg* cfg, double* transformation, double* fitness,
+             double* inlier_rmse, int32_t* iterations, void* stream);
+
 /* GPU Multiresolution IsoSurface Extraction (SURVEY §8f rank 4) — the class `mise.MISE` of code/src/libmise/mise.pyx (the
  * reference's only native code) as driven by generate_mesh (utils/meshing.py:9-72): same query / update / to_dense rounds,
  * same dense (R+1)^3 value grid, R = resolution_0 << depth, bit for bit; marching cubes stays with the caller (skimage).
