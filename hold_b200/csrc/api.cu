@@ -1376,13 +1376,19 @@ int hold_wgrad(hold_ctx* ctx, int P, const float* D, int ldd, int N, const float
   HOLD_REQUIRE(P >= 0 && N >= 1 && N <= 256 && K >= 1 && K <= 256 && ldd >= N && lda >= K && ldo >= K, "hold_wgrad: N, K in [1, 256]");
   HOLD_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t s = (cudaStream_t)stream;
-  HOLD_CUDA(cudaMemset2DAsync(out, (size_t)ldo * sizeof(float), 0, (size_t)K * sizeof(float), N, s));
-  if (P == 0) return HOLD_OK;
+  if (P == 0) {
+    HOLD_CUDA(cudaMemset2DAsync(out, (size_t)ldo * sizeof(float), 0, (size_t)K * sizeof(float), N, s));
+    return HOLD_OK;
+  }
+  // the partials' workspace has one size for every shape, so a captured call never sees it reallocated by a later call
+  WS(WS_WGRAD, uint8_t, kWgPartBytes, part);
   WgArgs a;
   a.P = P, a.N = N, a.K = K, a.ldd = ldd, a.lda = lda, a.ldo = ldo, a.D = D, a.A = A, a.d_scale = d_scale, a.a_scale = a_scale;
-  a.out = out, a.err = ctx->dev_err;
-  const int slabs = ceil_div(P, kWgPts), nblk = ceil_div(N, kWgRowsD);
-  k_wgrad_tc<<<dim3(max(1, min(slabs, ctx->sm_count / nblk)), nblk), kWgThreads, kWgSmem, s>>>(a);
+  a.part = (float*)part, a.out = out, a.err = ctx->dev_err;
+  const int splits = wgrad_splits(P, N);
+  k_wgrad_tc<<<dim3(splits, ceil_div(N, kWgRowsD)), kWgThreads, kWgSmem, s>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_wgrad_sum<<<ceil_div(N * K, 32), kWgSumWarps * 32, 0, s>>>(a.part, splits, N, K, out, ldo);
   HOLD_LAUNCH_CHECK(ctx);
   return HOLD_OK;
 }

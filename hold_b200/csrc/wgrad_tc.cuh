@@ -1,4 +1,4 @@
-// Weight-gradient reduction of the training backward on the tensor cores (SURVEY §8f rank 2): OUT[n, k] += sum_p D[p, n] * A[p, k]
+// Weight-gradient reduction of the training backward on the tensor cores (SURVEY §8f rank 2): OUT[n, k] = sum_p D[p, n] * A[p, k]
 // for row-major fp32 D [P, N <= 256] (a pre-activation gradient) and A [P, K <= 256] (the layer's input), fp32-level arithmetic.
 //
 // The contraction runs over the POINTS, so both MMA operands are the transposes D^T [n x p] and A^T [k x p]: the 8 warps read
@@ -7,9 +7,12 @@
 // stores one 16-byte unit of the K-major SW64 canonical layout — the transposition happens in registers, the smem images are the
 // same layout the weight stages of mlp_tc.cuh use.  Each CTA owns one 128-row block of n (blockIdx.y); its two warpgroups issue
 // wgmma m64n256k16 (64 rows of n each, all 256 columns of k, K = 16 points, 3 passes hi*hi + lo*hi + hi*lo) into register
-// accumulators while the next slab is loaded into the other half of a 2-stage smem ring.  Every CTA sweeps its share of the point
-// slabs, then adds its partial to OUT with red.global.add.f32 (the order of those adds is not fixed: fp32 round-off level, far
-// below the 1e-4 gradient bar).
+// accumulators while the next slab is loaded into the other half of a 2-stage smem ring.
+//
+// Fixed-order split reduction: split s = blockIdx.x sweeps slabs s, s + S, s + 2S, ... and stores its partial [N, K] (row-major)
+// into the context's WS_WGRAD workspace; k_wgrad_sum then adds the S partials of each element in an order that depends on S alone
+// and stores OUT once.  S = min(slabs, kWgSplitCtas / n-blocks) depends only on (P, N) — not on the SM count — so the result is
+// the same bits on every run and every Hopper part.  No floating-point atomics.
 #pragma once
 #include "mlp_tc.cuh"
 
@@ -23,6 +26,16 @@ constexpr int kWgStage = 2 * kWgImgD + 2 * kWgImgA;   // D^T hi | D^T lo | A^T h
 constexpr int kWgStages = 2;
 constexpr int kWgThreads = 256;
 constexpr int kWgSmem = kWgStages * kWgStage + 1024;
+// CTAs of one launch at most (split count x n-blocks): a constant, so that the split count and with it the order of the sums
+// does not depend on the GPU; one CTA per SM, so one wave on an H100 SXM's 132 SMs (fewer splits leave SMs idle)
+constexpr int kWgSplitCtas = 132;
+// partials of one call: S * N * K floats, at most 132 splits x 128 rows (one n-block) or 66 x 256 (two), K <= 256
+constexpr size_t kWgPartBytes = (size_t)kWgSplitCtas * kWgRowsD * 256 * sizeof(float);   // 16.5 MiB
+constexpr int kWgSumWarps = 8;                  // k_wgrad_sum: warps per CTA, each adds a contiguous run of the splits
+
+__host__ __device__ inline int wgrad_splits(int P, int N) {
+  return min(ceil_div(P, kWgPts), kWgSplitCtas / ceil_div(N, kWgRowsD));
+}
 
 struct WgArgs {
   int P, N, K, ldd, lda, ldo;
@@ -30,6 +43,7 @@ struct WgArgs {
   const float* A;
   const float* d_scale;   // device scalars (powers of two) or NULL
   const float* a_scale;
+  float* part;            // [gridDim.x][N][K] partials (WS_WGRAD)
   float* out;
   int* err;
 };
@@ -47,6 +61,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) k_wgrad_tc(WgArgs a) {
   const int n0 = blockIdx.y * kWgRowsD;
   const int n_slabs = ceil_div(a.P, kWgPts);
   const int my_slabs = (n_slabs > (int)blockIdx.x) ? (n_slabs - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  // never taken (hold_wgrad launches at most one split per slab), but without this exit ptxas schedules the slab loop differently
+  // and the kernel runs 40 % slower (H100 SXM, P = 125 440, N = K = 256)
   if (my_slabs == 0) return;
   const float dsc = kTcScaleA / ((a.d_scale != nullptr) ? __ldg(a.d_scale) : 1.0f);
   const float asc = kTcScaleW / ((a.a_scale != nullptr) ? __ldg(a.a_scale) : 1.0f);
@@ -104,6 +120,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) k_wgrad_tc(WgArgs a) {
   }
   wgmma_wait<0>();
   // ============================================================ accumulator read-out: rows n of this warpgroup, columns k
+  float* part = a.part + (size_t)blockIdx.x * a.N * a.K;
   const float osc = ((a.d_scale != nullptr) ? __ldg(a.d_scale) : 1.0f) * ((a.a_scale != nullptr) ? __ldg(a.a_scale) : 1.0f) /
                     (kTcScaleA * kTcScaleW);
   const int nr = n0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -116,9 +133,31 @@ __global__ void __launch_bounds__(kWgThreads, 1) k_wgrad_tc(WgArgs a) {
 #pragma unroll
       for (int t = 0; t < 2; ++t) {
         const int k = 8 * j + 2 * (lane & 3) + t;
-        if (k < a.K) atomicAdd(a.out + (size_t)n * a.ldo + k, acc[4 * j + 2 * h + t] * osc);
+        if (k < a.K) part[(size_t)n * a.K + k] = acc[4 * j + 2 * h + t] * osc;
       }
     }
+  }
+}
+
+// OUT[n, k] = sum of the S partials of element e = n * K + k.  Each CTA takes 32 consecutive elements (lane = element); warp w adds
+// the splits [w * c, (w + 1) * c) in ascending order (c = ceil(S / 8)), then warp 0 adds the eight runs in warp order.
+__global__ void __launch_bounds__(kWgSumWarps * 32) k_wgrad_sum(const float* __restrict__ part, int S, int N, int K, float* out,
+                                                                 int ldo) {
+  __shared__ float run[kWgSumWarps][32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nk = N * K, e = blockIdx.x * 32 + lane;
+  const int c = ceil_div(S, kWgSumWarps), s1 = min(S, (warp + 1) * c);
+  float v = 0.f;
+  if (e < nk) {
+#pragma unroll 8
+    for (int s = warp * c; s < s1; ++s) v += __ldcg(part + (size_t)s * nk + e);
+  }
+  run[warp][lane] = v;
+  __syncthreads();
+  if (warp == 0 && e < nk) {
+#pragma unroll
+    for (int w = 1; w < kWgSumWarps; ++w) v += run[w][lane];
+    out[(size_t)(e / K) * ldo + e % K] = v;
   }
 }
 

@@ -366,7 +366,12 @@ int hold_linear(hold_ctx* ctx, int node, int mat, int P, const float* A, int lda
 
 /* Weight-gradient reduction over the points, out[n, k] = sum_p D[p, n] * A[p, k] (N, K <= 256; out [N, ldo] is overwritten), on
  * wgmma with the same fp16 hi/lo split x 3 passes (hold_b200/csrc/wgrad_tc.cuh).  d_scale / a_scale: device scalars (powers of
- * two, NULL = 1) by which D / A are divided before the split; the result is multiplied back. */
+ * two, NULL = 1) by which D / A are divided before the split; the result is multiplied back.
+ * Bitwise reproducible: the points are split into a number of ranges that depends on P and N only, each range's partial sum goes
+ * to a context-owned workspace, and a second kernel adds the partials in a fixed order (no floating-point atomics).  The same
+ * inputs give the same bits on every call, eager or replayed from a CUDA graph, on any sm_90a part.  The workspace (16.5 MiB) is
+ * allocated by the context's first call with P > 0, so make one such call before capturing a graph; after that it is never
+ * reallocated.  All calls on one context share it: issue them on one stream (or order them across streams). */
 int hold_wgrad(hold_ctx* ctx, int P, const float* D, int ldd, int N, const float* A, int lda, int K, const float* d_scale,
                const float* a_scale, float* out, int ldo, void* stream);
 
