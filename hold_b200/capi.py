@@ -107,6 +107,7 @@ EXPORTS = {
     "hold_raster_silhouette_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_int, fp, C.c_int, C.c_int, C.POINTER(RasterCfg),
                                              fp, fp, C.c_void_p]),
     "hold_knn_points": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, C.c_int, fp, fp, C.c_int, fp, fp, C.c_void_p]),
+    "hold_knn_points_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, C.c_int, fp, fp, C.c_int, fp, fp, fp, fp, fp, C.c_void_p]),
     "hold_icp": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, C.c_int, fp, fp, fp, C.POINTER(IcpCfg), fp, fp, fp, fp, C.c_void_p]),
     "hold_mano_lbs_bwd": (C.c_int, [C.c_void_p, C.POINTER(ManoModel), C.c_int] + [fp] * 12 + [C.c_void_p]),
     "hold_object_tf_bwd": (C.c_int, [C.c_void_p, C.c_int, fp, fp, fp, C.c_float, fp, fp, C.c_int] + [fp] * 6 + [C.c_void_p]),

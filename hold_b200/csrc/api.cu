@@ -941,9 +941,25 @@ int hold_raster_silhouette_bwd(hold_ctx* ctx, int B, int V, const float* verts_n
   RasterArgs a;
   int rc = raster_setup(ctx, B, V, verts_ndc, F, faces, H, W, cfg, &a, stream);
   if (rc || B == 0) return rc;
-  a.g_sil = g_sil, a.g_verts = g_verts;
-  HOLD_CUDA(cudaMemsetAsync(g_verts, 0, sizeof(float) * (size_t)B * V * 3, (cudaStream_t)stream));
-  k_raster<true><<<dim3(ceil_div(H, kRasterTile) * ceil_div(W, kRasterTile), B), kRasterThreads, 0, (cudaStream_t)stream>>>(a);
+  cudaStream_t s = (cudaStream_t)stream;
+  // one workspace, sized from the arguments: Q and thresholds per pixel, the faces' partials, the vertex map
+  const size_t npix = (size_t)B * H * W, o_q = npix * sizeof(uint64_t), o_part = (o_q + npix * sizeof(float) + 255) & ~(size_t)255;
+  const size_t o_keys = (o_part + (size_t)B * F * kRbPieces * 6 * sizeof(float) + 255) & ~(size_t)255;
+  const size_t o_map = o_keys + (((size_t)F * 3 * sizeof(int) + 255) & ~(size_t)255);
+  WS(WS_RASTER_BWD, uint8_t, o_map + inverse_map_ints(F * 3, V) * sizeof(int), ws);
+  a.thr = (uint64_t*)ws, a.q = (float*)(ws + o_q);
+  k_raster<true><<<dim3(ceil_div(H, kRasterTile) * ceil_div(W, kRasterTile), B), kRasterThreads, 0, s>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  RasterBwdArgs g;
+  g.V = V, g.F = F, g.H = H, g.W = W, g.fbits = a.fbits, g.o = a.o;
+  g.rec = a.rec, g.q = a.q, g.thr = a.thr, g.g_sil = g_sil, g.part = (float*)(ws + o_part), g.g_verts = g_verts;
+  int* keys = (int*)(ws + o_keys);
+  k_raster_vert_keys<<<ceil_div(F * 3, 256), 256, 0, s>>>(F * 3, V, faces, keys);
+  HOLD_LAUNCH_CHECK(ctx);
+  if ((rc = inverse_map(ctx, keys, F * 3, V, (int*)(ws + o_map), &g.vmap, s))) return rc;
+  k_raster_bwd_faces<<<dim3(F * (kRbPieces / kRbWarps), B), kRbWarps * 32, 0, s>>>(g);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_raster_bwd_verts<<<dim3(ceil_div(V, 128), B), 128, 0, s>>>(g);
   HOLD_LAUNCH_CHECK(ctx);
   return HOLD_OK;
 }
@@ -967,6 +983,39 @@ int hold_knn_points(hold_ctx* ctx, int N, int P1, const float* p1, const int32_t
   else if (K <= 16) HOLD_KNN_CASE(16);
   else HOLD_KNN_CASE(32);
 #undef HOLD_KNN_CASE
+  HOLD_LAUNCH_CHECK(ctx);
+  return HOLD_OK;
+}
+
+int hold_knn_points_bwd(hold_ctx* ctx, int N, int P1, const float* p1, const int32_t* lengths1, int P2, const float* p2,
+                        const int32_t* lengths2, int K, const int32_t* idx, const float* g_dists, const float* g_knn, float* g_p1,
+                        float* g_p2, void* stream) {
+  HOLD_REQUIRE(ctx != nullptr, "ctx is NULL");
+  HOLD_REQUIRE(N >= 0 && P1 >= 0 && P2 >= 0, "bad sizes N %d P1 %d P2 %d", N, P1, P2);
+  HOLD_REQUIRE(K >= 1 && K <= HOLD_KNN_MAX_K, "K %d outside [1, %d]", K, (int)HOLD_KNN_MAX_K);
+  HOLD_REQUIRE((int64_t)N * P1 * K < (1ll << 31) && (int64_t)N * P2 < (1ll << 31), "N P1 K = %lld or N P2 = %lld slots is over 2^31",
+               (long long)N * P1 * K, (long long)N * P2);
+  if (N == 0) return HOLD_OK;
+  HOLD_REQUIRE((P1 == 0 || (p1 && idx && g_dists && g_p1)) && (P2 == 0 || (p2 && g_p2)), "NULL argument");
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  const int S = N * P1 * K, T = N * P2;
+  KnnBwdArgs a{};
+  a.N = N, a.P1 = P1, a.P2 = P2, a.K = K, a.p1 = p1, a.p2 = p2, a.len1 = lengths1, a.len2 = lengths2, a.idx = idx;
+  a.g_dists = g_dists, a.g_knn = g_knn, a.g_p1 = g_p1, a.g_p2 = g_p2, a.err = ctx->dev_err;
+  // one workspace, sized from the arguments: the slots' p2 parts, their keys, the inverse map
+  const size_t o_keys = ((size_t)S * 3 * sizeof(float) + 255) & ~(size_t)255;
+  const size_t o_map = o_keys + (((size_t)S * sizeof(int) + 255) & ~(size_t)255);
+  WS(WS_KNN_BWD, uint8_t, o_map + inverse_map_ints(S, T) * sizeof(int), ws);
+  a.contrib = (float*)ws, a.keys = (int*)(ws + o_keys);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (S > 0) {
+    k_knn_bwd_rows<<<ceil_div(N * P1, kPcThreads), kPcThreads, 0, s>>>(a);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  if (T == 0) return HOLD_OK;
+  int rc = inverse_map(ctx, a.keys, S, T, (int*)(ws + o_map), &a.map, s);
+  if (rc) return rc;
+  k_knn_bwd_targets<<<ceil_div(T, kPcThreads), kPcThreads, 0, s>>>(a);
   HOLD_LAUNCH_CHECK(ctx);
   return HOLD_OK;
 }

@@ -52,7 +52,8 @@ struct PackedNet {
 
 // grow-only workspaces of a hold_ctx, one per purpose
 enum WsSlot { WS_Z = 0, WS_SDF, WS_ZNEW, WS_SDFNEW, WS_BETA, WS_FAR, WS_XC, WS_SSDF, WS_GRAD, WS_FEAT, WS_PE, WS_ZTMP, WS_SIG,
-              WS_BGSDF, WS_BGFEAT, WS_BGRGB, WS_AMAX, WS_WARPBWD, WS_RASTER, WS_ICP, WS_WGRAD, WS_COUNT };
+              WS_BGSDF, WS_BGFEAT, WS_BGRGB, WS_AMAX, WS_WARPBWD, WS_RASTER, WS_ICP, WS_WGRAD,
+              WS_RASTER_BWD, WS_KNN_BWD, WS_COUNT };
 
 struct NodeState {
   bool configured = false, has_weights = false, has_rig = false;

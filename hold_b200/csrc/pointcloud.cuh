@@ -10,10 +10,14 @@
 // rounds do (DESIGN.md §3.2), so the call can be captured in a CUDA graph.  Every sum over correspondences is a per-CTA
 // shuffle tree, then the CTAs' partials added in CTA order by one thread: bitwise reproducible, and a pair's bits do not
 // depend on the other pairs of the batch.
+//
+// The K-NN backward (hold_knn_points_bwd) adds in a fixed order with no atomic: a query's gradient sums its slots in k order,
+// and a target's gradient sums the slots that chose it in ascending (query, k) order, found through inverse_map.cuh.
 #pragma once
 #include <limits.h>
 
 #include "common.cuh"
+#include "inverse_map.cuh"
 #include "pointcloud_phases.h"
 
 namespace hold {
@@ -86,6 +90,73 @@ __global__ void __launch_bounds__(kPcThreads) k_knn(int N, int P1, const float* 
         }
     }
   }
+}
+
+// ---- K-NN backward
+
+struct KnnBwdArgs {
+  int N, P1, P2, K;
+  const float *p1, *p2;
+  const int *len1, *len2;
+  const int* idx;          // [N,P1,K] from k_knn
+  const float* g_dists;    // [N,P1,K]
+  const float* g_knn;      // [N,P1,K,3] or NULL
+  float *g_p1, *g_p2;      // [N,P1,3], [N,P2,3], overwritten
+  float* contrib;          // [N,P1,K,3]: each slot's d loss / d p2 through dists
+  int* keys;               // [N,P1,K]: n P2 + idx for a slot that reaches p2, else N P2
+  InvMap map;
+  int* err;
+};
+
+// One thread per query row: g_p1 = sum over the valid slots in k order of 2 (p1 - p2[idx]) g_dists; the slots' keys and p2
+// parts.  A slot reaches p2 through dists when it is valid (row < lengths1, k < lengths2), through knn when k < lengths2.
+__global__ void __launch_bounds__(kPcThreads) k_knn_bwd_rows(KnnBwdArgs a) {
+  const int64_t row = (int64_t)blockIdx.x * kPcThreads + threadIdx.x;
+  if (row >= (int64_t)a.N * a.P1) return;
+  const int n = (int)(row / a.P1), i = (int)(row % a.P1);
+  const bool report = row == 0;
+  const int L1 = pc_length(a.len1, n, a.P1, a.err, report), L2 = pc_length(a.len2, n, a.P2, a.err, report);
+  const float* q = a.p1 + row * 3;
+  float g1[3] = {0.f, 0.f, 0.f};
+  for (int k = 0; k < a.K; ++k) {
+    const int64_t slot = row * a.K + k;
+    const int j = a.idx[slot];
+    const bool in = k < L2 && j >= 0 && j < L2, vd = in && i < L1;
+    float c[3] = {0.f, 0.f, 0.f};
+    if (vd) {
+      const float* t = a.p2 + ((size_t)n * a.P2 + j) * 3;
+      const float gd = a.g_dists[slot];
+#pragma unroll
+      for (int e = 0; e < 3; ++e) {
+        const float d = __fmul_rn(2.f * (q[e] - t[e]), gd);
+        g1[e] += d;
+        c[e] = -d;
+      }
+    }
+    a.keys[slot] = vd || (in && a.g_knn) ? n * a.P2 + j : a.N * a.P2;
+#pragma unroll
+    for (int e = 0; e < 3; ++e) a.contrib[slot * 3 + e] = c[e];
+  }
+#pragma unroll
+  for (int e = 0; e < 3; ++e) a.g_p1[row * 3 + e] = g1[e];
+}
+
+// One thread per target: the slots that chose it, in ascending (query, k) order; the dists part and the knn part are summed
+// apart and added last.
+__global__ void __launch_bounds__(kPcThreads) k_knn_bwd_targets(KnnBwdArgs a) {
+  const int t = blockIdx.x * kPcThreads + threadIdx.x;
+  if (t >= a.N * a.P2) return;
+  float sd[3] = {0.f, 0.f, 0.f}, sk[3] = {0.f, 0.f, 0.f};
+  for (int e = a.map.first[t]; e < a.map.first[t + 1]; ++e) {
+    const size_t slot = a.map.order[e];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      sd[c] += a.contrib[slot * 3 + c];
+      if (a.g_knn) sk[c] += a.g_knn[slot * 3 + c];
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) a.g_p2[(size_t)t * 3 + c] = a.g_knn ? sd[c] + sk[c] : sd[c];
 }
 
 // ---- ICP

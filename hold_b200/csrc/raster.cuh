@@ -5,13 +5,21 @@
 // order (ballot), and every thread tests its pixel against them.  Per pixel the forward keeps the candidate count and the
 // product Q of (1 - p).  When some pixel of the tile has more than K candidates, the tile bisects that pixel's K-th key
 // (pz, face) bit by bit, one pass over the faces per bit, and redoes the product over the keys <= it: the selection is exact
-// and nothing of size K per pixel is stored.  The backward recomputes the selection the same way.
+// and nothing of size K per pixel is stored.  The silhouette is bitwise reproducible: each pixel multiplies its factors in
+// face order.
 //
-// The backward accumulates the vertex gradients with fp32 atomics (per chunk in shared memory, then into g_verts): the
-// gradient is not bitwise reproducible from run to run.  The silhouette is: each pixel multiplies its factors in face order.
+// The backward adds in an order fixed by the inputs alone, with no atomic, so g_verts is bitwise reproducible and a frame's
+// bits do not depend on the rest of the batch:
+//   1. k_raster<true> recomputes the selection the same way and stores each pixel's Q and key threshold ([B,H,W] each);
+//   2. k_raster_bwd_faces runs one warp per (frame, face, piece of the face's pixel box): the warp re-tests the piece's pixels
+//      (pixel_face, key <= threshold), each lane adds its pixels' vertex-xy gradients in row-major order, a shuffle tree adds
+//      the lanes, and lane 0 stores the piece's 6 sums ([B,F,kRbPieces,6]);
+//   3. k_raster_bwd_verts sums, per vertex, its (face, corner) partials in ascending face order, then piece order: the
+//      inverse of faces comes from inverse_map.cuh.
 #pragma once
 #include "common.cuh"
 #include "raster_phases.h"
+#include "inverse_map.cuh"
 
 namespace hold {
 
@@ -58,8 +66,8 @@ struct RasterArgs {
   int64_t* p2f;        // forward, optional (all three or none): [B, H, W, K]
   float* zbuf;
   float* dists;
-  const float* g_sil;  // backward: [B, H, W] -> g_verts [B, V, 3] (accumulated; x and y only)
-  float* g_verts;
+  float* q;            // backward: per pixel, Q and the selection's key threshold [B, H, W]
+  uint64_t* thr;
 };
 
 template <bool kBwd>
@@ -67,7 +75,6 @@ __global__ void __launch_bounds__(kRasterThreads) k_raster(RasterArgs a) {
   constexpr int kWarps = kRasterThreads / 32;
   __shared__ int s_list[kRasterThreads];                  // this chunk's faces that overlap the tile, in face order
   __shared__ int s_wcnt[kWarps];
-  __shared__ float s_g[kBwd ? kRasterThreads * 6 : 1];   // backward: the chunk's vertex-xy gradients
   const int b = blockIdx.y, ntx = ceil_div(a.W, kRasterTile);
   const int i0 = (blockIdx.x / ntx) * kRasterTile, j0 = (blockIdx.x % ntx) * kRasterTile;
   const int i = i0 + threadIdx.x / kRasterTile, j = j0 + threadIdx.x % kRasterTile;
@@ -170,33 +177,106 @@ __global__ void __launch_bounds__(kRasterThreads) k_raster(RasterArgs a) {
         a.p2f[base + pos] = fb + f, a.zbuf[base + pos] = fr.pz, a.dists[base + pos] = raster::signed_dist(fr);
       }, nothing);
     }
-  } else {
-    const float g = live ? a.g_sil[pix] : 0.f;
-    const bool act = live && g != 0.f && Q != 0.f;   // Q = 0: every kept face's gradient is 0 (raster_phases.h)
-    if (__syncthreads_or(act)) {
-      for (int k = threadIdx.x; k < kRasterThreads * 6; k += kRasterThreads) s_g[k] = 0.f;
-      pass([&](int slot, int f) {
-        raster::Frag fr;
-        if (!act || !test(f, fr) || raster::frag_key(fr.pz, f, a.fbits) > thr) return;
-        const float gd = raster::blend_ddist(g, Q, fr, a.o.sigma);
-        if (gd == 0.f) return;
-        float gv[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        raster::tri_sqdist_bwd(px, py, v, fr.edge, gd, gv);
-        for (int c = 0; c < 6; ++c)
-          if (gv[c] != 0.f) atomicAdd(&s_g[slot * 6 + c], gv[c]);
-      }, [&](int n) {
-        __syncthreads();
-        for (int k = threadIdx.x; k < n * 6; k += kRasterThreads) {
-          const float x = s_g[k];
-          if (x == 0.f) continue;
-          s_g[k] = 0.f;
-          const float4 r3 = rec[(size_t)s_list[k / 6] * 4 + 3];
-          const int c = k % 6, vid = __float_as_int(c < 2 ? r3.y : c < 4 ? r3.z : r3.w);
-          atomicAdd(&a.g_verts[((size_t)b * a.V + vid) * 3 + (c & 1)], x);
-        }
-      });
-    }
+  } else if (live) {
+    a.q[pix] = Q, a.thr[pix] = thr;
   }
+}
+
+constexpr int kRbWarps = 8;            // pieces per CTA of k_raster_bwd_faces
+constexpr int kRbPieces = 16;          // the most pieces a face's pixel box is split into
+constexpr int kRbPiecePixels = 256;    // the fewest pixels a piece is given when the box allows it
+
+// Pixels whose centre may lie inside a face's expanded box (record word 0), with a pixel of margin; pixel_face still decides.
+// An empty box gives no pixel, a NaN box the whole image.
+struct PixBox {
+  int i0, j0, ni, nj;
+};
+__device__ __forceinline__ PixBox pix_box(float4 bb, int H, int W) {
+  const float s = (float)min(H, W);
+  // pix_ndc(j) = (W - 2j - 1) / s decreases with j: x <= xmax  <=>  j >= (W - 1 - xmax s) / 2
+  const float j0 = fmaxf(floorf((W - 1 - bb.y * s) * 0.5f) - 1.f, 0.f), j1 = fminf(ceilf((W - 1 - bb.x * s) * 0.5f) + 1.f, W - 1.f);
+  const float i0 = fmaxf(floorf((H - 1 - bb.w * s) * 0.5f) - 1.f, 0.f), i1 = fminf(ceilf((H - 1 - bb.z * s) * 0.5f) + 1.f, H - 1.f);
+  if (!(j0 <= j1 && i0 <= i1)) return PixBox{0, 0, 0, 0};
+  return PixBox{(int)i0, (int)j0, (int)(i1 - i0) + 1, (int)(j1 - j0) + 1};
+}
+// pieces of a box: one per kRbPiecePixels pixels, 1 .. kRbPieces (an empty box has one piece, with no pixel)
+__device__ __forceinline__ int pix_pieces(const PixBox& p) {
+  const int64_t n = ((int64_t)p.ni * p.nj + kRbPiecePixels - 1) / kRbPiecePixels;
+  return n < 1 ? 1 : n > kRbPieces ? kRbPieces : (int)n;
+}
+
+struct RasterBwdArgs {
+  int V, F, H, W, fbits;
+  raster::Opts o;
+  const float4* rec;     // [B, F, 4] from k_raster_setup
+  const float* q;        // [B, H, W] from k_raster<true>
+  const uint64_t* thr;
+  const float* g_sil;    // [B, H, W]
+  float* part;           // [B, F, kRbPieces, 6]: each face's vertex-xy gradients per piece (the first pix_pieces are written)
+  InvMap vmap;           // faces inverted: item 3 f + c, key = vertex id
+  float* g_verts;        // [B, V, 3], overwritten (x and y; z = 0)
+};
+
+// grid (F * kRbPieces / kRbWarps, B), kRbWarps warps: one warp per (frame, face, piece)
+__global__ void __launch_bounds__(kRbWarps * 32) k_raster_bwd_faces(RasterBwdArgs a) {
+  const int b = blockIdx.y, f = blockIdx.x / (kRbPieces / kRbWarps);
+  const int piece = (blockIdx.x % (kRbPieces / kRbWarps)) * kRbWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  const float4* r = a.rec + ((size_t)b * a.F + f) * 4;
+  const float4 r0 = r[0];
+  const PixBox pb = pix_box(r0, a.H, a.W);
+  const int np = pix_pieces(pb);
+  if (piece >= np) return;   // warp-uniform
+  const float4 r1 = r[1], r2 = r[2], r3 = r[3];
+  const float bb[4] = {r0.x, r0.y, r0.z, r0.w};
+  const float v[9] = {r1.x, r1.y, r1.z, r1.w, r2.x, r2.y, r2.z, r2.w, r3.x};
+  const int s = min(a.H, a.W);
+  const int64_t n = (int64_t)pb.ni * pb.nj, p1 = n * (piece + 1) / np;
+  const size_t frame = (size_t)b * a.H * a.W;
+  float gv[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int64_t p = n * piece / np + lane; p < p1; p += 32) {
+    const int i = pb.i0 + (int)(p / pb.nj), j = pb.j0 + (int)(p % pb.nj);
+    const size_t pix = frame + (size_t)i * a.W + j;
+    const float g = a.g_sil[pix], Q = a.q[pix];
+    if (g == 0.f || Q == 0.f) continue;   // Q = 0: every kept face's gradient is 0 (raster_phases.h)
+    const float px = raster::pix_ndc(j, a.W, s), py = raster::pix_ndc(i, a.H, s);
+    raster::Frag fr;
+    if (!raster::pixel_face(v, bb, px, py, a.o, fr) || raster::frag_key(fr.pz, f, a.fbits) > a.thr[pix]) continue;
+    const float gd = raster::blend_ddist(g, Q, fr, a.o.sigma);
+    if (gd != 0.f) raster::tri_sqdist_bwd(px, py, v, fr.edge, gd, gv);
+  }
+#pragma unroll
+  for (int c = 0; c < 6; ++c)
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) gv[c] += __shfl_down_sync(0xffffffffu, gv[c], off);
+  if (lane == 0) {
+    float* out = a.part + (((size_t)b * a.F + f) * kRbPieces + piece) * 6;
+#pragma unroll
+    for (int c = 0; c < 6; ++c) out[c] = gv[c];
+  }
+}
+
+// grid (ceil(V / 128), B), 128 threads: one thread per (frame, vertex)
+__global__ void __launch_bounds__(128) k_raster_bwd_verts(RasterBwdArgs a) {
+  const int vid = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+  if (vid >= a.V) return;
+  float sx = 0.f, sy = 0.f;
+  for (int e = a.vmap.first[vid]; e < a.vmap.first[vid + 1]; ++e) {
+    const int item = a.vmap.order[e], f = item / 3, c = item % 3;
+    const size_t fb = (size_t)b * a.F + f;
+    const int np = pix_pieces(pix_box(a.rec[fb * 4], a.H, a.W));
+    const float* p = a.part + fb * kRbPieces * 6 + 2 * c;
+    for (int k = 0; k < np; ++k) sx += p[k * 6], sy += p[k * 6 + 1];
+  }
+  float* g = a.g_verts + ((size_t)b * a.V + vid) * 3;
+  g[0] = sx, g[1] = sy, g[2] = 0.f;
+}
+
+// keys of the (face, corner) items for inverse_map: the vertex id, or V for an index outside [0, V)
+__global__ void k_raster_vert_keys(int n, int V, const int* __restrict__ faces, int* __restrict__ keys) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const int id = faces[e];
+  keys[e] = id >= 0 && id < V ? id : V;
 }
 
 }  // namespace hold

@@ -57,11 +57,13 @@ def _valid(l1, l2, P1, K):
 
 
 class KnnPointsFn(torch.autograd.Function):
-    """dists [N,P1,K] (squared, differentiable in p1 and p2) and idx [N,P1,K] int32 of hold_knn_points; the backward is
-    pytorch3d's: g_p1 += 2 (p1 - p2[idx]) g, g_p2[idx] -= the same, over the valid slots."""
+    """dists [N,P1,K] (squared, differentiable in p1 and p2) and idx [N,P1,K] int32 of hold_knn_points, and with return_nn
+    knn [N,P1,K,3] = p2[idx] in p2's dtype, zero in the slots k >= lengths2 (pytorch3d's knn_gather, differentiable in p2).
+    The backward is pytorch3d's on hold_knn_points_bwd: g_p1 += 2 (p1 - p2[idx]) g, g_p2[idx] -= the same over the valid
+    slots, plus knn's gradient at idx; every sum in a fixed order (bitwise reproducible), accumulated in fp32."""
 
     @staticmethod
-    def forward(fctx, p1, p2, l1, l2, K, ctx):
+    def forward(fctx, p1, p2, l1, l2, K, ctx, return_nn=False):
         a, b = p1.detach().float().contiguous(), p2.detach().float().contiguous()
         N, P1, _ = a.shape
         P2 = b.shape[1]
@@ -70,40 +72,66 @@ class KnnPointsFn(torch.autograd.Function):
         check(lib().hold_knn_points(ctx.h, N, P1, ptr(a), ptr(l1), P2, ptr(b), ptr(l2), K, ptr(dists), ptr(idx), stream_ptr()))
         fctx.save_for_backward(a, b, l1, l2, idx)
         fctx.mark_non_differentiable(idx)
-        fctx.dtypes = (p1.dtype, p2.dtype)
-        return dists, idx
+        fctx.dtypes, fctx.ctx, fctx.return_nn = (p1.dtype, p2.dtype), ctx, return_nn
+        if not return_nn:
+            return dists, idx
+        if P2 == 0:
+            knn = p2.new_zeros(N, P1, K, 3)
+        else:
+            knn = torch.gather(p2.detach(), 1, idx.long().reshape(N, P1 * K, 1).expand(-1, -1, 3)).reshape(N, P1, K, 3)
+            knn = knn * (torch.arange(K, device=p1.device)[None, None, :] < l2[:, None, None])[..., None]
+        return dists, idx, knn
 
     @staticmethod
-    def backward(fctx, g_dists, _g_idx):
+    def backward(fctx, g_dists, _g_idx, g_knn=None):
         a, b, l1, l2, idx = fctx.saved_tensors
         N, P1, K = idx.shape
         P2 = b.shape[1]
-        g1 = torch.zeros(N, P1, 3, device=a.device, dtype=a.dtype)
-        g2 = torch.zeros(N * P2, 3, device=b.device, dtype=b.dtype)
-        if P1 > 0 and P2 > 0:
+        gd = g_dists.float().contiguous()
+        gk = g_knn.float().contiguous() if g_knn is not None and P2 > 0 else None
+        if a.is_cuda:
+            g1 = torch.empty(N, P1, 3, device=a.device)
+            g2 = torch.empty(N, P2, 3, device=b.device)
             # only the valid slots contribute: padding rows of p1 and padding slots (which hold index 0, or address an empty p2)
-            # are selected away, so whatever they hold (inf, NaN) does not reach the gradients
-            ok = _valid(l1, l2, P1, K)[..., None]
-            il = idx.long()
-            nn = torch.gather(b, 1, il.reshape(N, P1 * K, 1).expand(-1, -1, 3)).reshape(N, P1, K, 3)
-            diff = torch.where(ok, 2.0 * (a[:, :, None, :] - nn) * g_dists[..., None], torch.zeros((), device=a.device))
-            g1 = diff.sum(2)
-            flat = (il + (torch.arange(N, device=b.device) * P2)[:, None, None]).reshape(-1)
-            g2.index_add_(0, flat, -diff.reshape(-1, 3))
-        return g1.to(fctx.dtypes[0]), g2.reshape(N, P2, 3).to(fctx.dtypes[1]), None, None, None, None
+            # are selected away on the device, so whatever they hold (inf, NaN) does not reach the gradients
+            check(lib().hold_knn_points_bwd(fctx.ctx.h, N, P1, ptr(a), ptr(l1), P2, ptr(b), ptr(l2), K, ptr(idx), ptr(gd), ptr(gk),
+                                            ptr(g1), ptr(g2), stream_ptr()))
+        else:
+            g1, g2 = _knn_backward_host(a, b, l1, l2, idx, gd, gk)
+        return g1.to(fctx.dtypes[0]), g2.to(fctx.dtypes[1]), None, None, None, None, None
 
 
-def _knn(ctx, p1, p2, l1, l2, K):
-    """(dists, idx int64) of KnnPointsFn for lengths that _check_lengths has already checked."""
-    dists, idx = KnnPointsFn.apply(p1, p2, l1, l2, K, ctx)
-    return dists, idx.long()
+def _knn_backward_host(a, b, l1, l2, idx, gd, gk):
+    """hold_knn_points_bwd's rules in torch ops for host tensors, whose index_add_ adds in index order."""
+    N, P1, K = idx.shape
+    P2 = b.shape[1]
+    g1, g2 = torch.zeros(N, P1, 3), torch.zeros(N * P2, 3)
+    if P1 > 0 and P2 > 0:
+        ok = _valid(l1, l2, P1, K)[..., None]
+        il = idx.long()
+        nn = torch.gather(b, 1, il.reshape(N, P1 * K, 1).expand(-1, -1, 3)).reshape(N, P1, K, 3)
+        diff = torch.where(ok, 2.0 * (a[:, :, None, :] - nn) * gd[..., None], torch.zeros(()))
+        g1 = diff.sum(2)
+        flat = (il + (torch.arange(N) * P2)[:, None, None]).reshape(-1)
+        g2.index_add_(0, flat, -diff.reshape(-1, 3))
+        if gk is not None:
+            kmask = (torch.arange(K)[None, None, :] < l2[:, None, None])[..., None]
+            g2.index_add_(0, flat, torch.where(kmask, gk, torch.zeros(())).reshape(-1, 3))
+    return g1, g2.reshape(N, P2, 3)
+
+
+def _knn(ctx, p1, p2, l1, l2, K, return_nn=False):
+    """(dists, idx int64[, knn]) of KnnPointsFn for lengths that _check_lengths has already checked."""
+    out = KnnPointsFn.apply(p1, p2, l1, l2, K, ctx, return_nn)
+    return (out[0], out[1].long()) + tuple(out[2:])
 
 
 def knn_points(ctx, p1, p2, lengths1=None, lengths2=None, K=1, return_nn=False):
     """pytorch3d.ops.knn_points (v0.7.4 rules, D = 3) on hold_knn_points: p1 [N,P1,3], p2 [N,P2,3] -> KNN(dists [N,P1,K]
     squared and ascending, idx [N,P1,K] int64, knn [N,P1,K,3] or None).  Ties go to the lower index; padding slots (row >=
     lengths1[n] or k >= lengths2[n]) hold 0.  dists is float32 whatever the inputs' dtype: the kernel computes in fp32 (its
-    gradients come back in the inputs' dtypes).  dists is differentiable in p1 and p2 (knn too, through torch.gather).  Checks
+    gradients come back in the inputs' dtypes).  dists is differentiable in p1 and p2, knn in p2; the backward is bitwise
+    reproducible (hold_knn_points_bwd).  Checks
     the lengths on the host first (one stream synchronisation when lengths are given)."""
     _cloud(p1, "p1"), _cloud(p2, "p2")
     if p1.shape[0] != p2.shape[0]:
@@ -112,14 +140,10 @@ def knn_points(ctx, p1, p2, lengths1=None, lengths2=None, K=1, return_nn=False):
         raise ValueError(f"K {K} outside [1, {KNN_MAX_K}]")
     N, P1, P2 = p1.shape[0], p1.shape[1], p2.shape[1]
     l1, l2 = _check_lengths(((lengths1, P1, "lengths1"), (lengths2, P2, "lengths2")), N, p1.device)
+    if return_nn:   # pytorch3d's knn_gather (zeros in the slots k >= lengths2), its gradient in the same fixed-order sum
+        return KNN(*_knn(ctx, p1, p2, l1, l2, K, True))
     dists, idx = _knn(ctx, p1, p2, l1, l2, K)
-    knn = None
-    if return_nn and P2 == 0:
-        knn = p2.new_zeros(N, P1, K, 3)
-    elif return_nn:   # pytorch3d's knn_gather: zeros in the slots k >= lengths2
-        knn = torch.gather(p2, 1, idx.reshape(N, P1 * K, 1).expand(-1, -1, 3)).reshape(N, P1, K, 3)
-        knn = knn * (torch.arange(K, device=p1.device)[None, None, :] < l2[:, None, None])[..., None]
-    return KNN(dists, idx, knn)
+    return KNN(dists, idx, None)
 
 
 def chamfer_distance(ctx, x, y, x_lengths=None, y_lengths=None, x_normals=None, y_normals=None, weights=None,

@@ -184,8 +184,10 @@ int hold_off_in_surface(hold_ctx* ctx, int R, int S, const float* sdf, float thr
  *   [B,H,W,K] are pytorch3d's fragments sorted by pz with -1 in empty slots; all three or none (NULL: nothing of size K per
  *   pixel is written or allocated).
  *   hold_raster_silhouette_bwd: g_sil [B,H,W] -> g_verts [B,V,3] (overwritten; x and y only: z, the selection and the culling
- *   carry no gradient, as in pytorch3d).  Accumulated with fp32 atomics, so not bitwise reproducible; recomputes the
- *   selection rather than storing it. */
+ *   carry no gradient, as in pytorch3d).  Recomputes the selection rather than storing it.  Every sum runs in an order fixed
+ *   by the inputs alone, with no atomic: g_verts is bitwise reproducible, and a frame's bits are the same alone or in a batch.
+ *   Its workspace is sized from the arguments (no device-to-host read): after one eager call with the same sizes (or larger),
+ *   the call can be captured in a CUDA graph, and the context's calls must not run on two streams at once. */
 enum { HOLD_RASTER_MAX_K = 1024 };
 typedef struct hold_raster_cfg {
   int32_t faces_per_pixel;         /* K, 1 .. HOLD_RASTER_MAX_K */
@@ -209,6 +211,16 @@ int hold_raster_silhouette_bwd(hold_ctx* ctx, int B, int V, const float* verts_n
 enum { HOLD_KNN_MAX_K = 32 };
 int hold_knn_points(hold_ctx* ctx, int N, int P1, const float* p1, const int32_t* lengths1, int P2, const float* p2,
                     const int32_t* lengths2, int K, float* dists, int32_t* idx, void* stream);
+/*   hold_knn_points_bwd: pytorch3d's knn_points backward at hold_knn_points' idx.  g_dists [N,P1,K] -> g_p1 [N,P1,3] =
+ *   sum over k of 2 (p1 - p2[idx]) g_dists, g_p2 [N,P2,3] = minus the same, at idx; both over the valid slots only (row <
+ *   lengths1[n], k < lengths2[n]).  g_knn [N,P1,K,3] (nullable) is the gradient of knn_gather's output p2[idx] with its
+ *   slots k >= lengths2[n] zeroed: it adds to g_p2 at idx from every slot k < lengths2[n].  Both outputs are overwritten.
+ *   Every sum runs in an order fixed by the inputs alone, with no atomic: a target sums the slots that chose it in ascending
+ *   (query, k) order, so the result is bitwise reproducible.  N P1 K and N P2 below 2^31.  Workspace and capture as
+ *   hold_raster_silhouette_bwd. */
+int hold_knn_points_bwd(hold_ctx* ctx, int N, int P1, const float* p1, const int32_t* lengths1, int P2, const float* p2,
+                        const int32_t* lengths2, int K, const int32_t* idx, const float* g_dists, const float* g_knn, float* g_p1,
+                        float* g_p2, void* stream);
 /*   hold_icp: open3d registration_icp with TransformationEstimationPointToPoint(with_scaling) for N independent pairs
  *   (source [N,Ps,3], target [N,Pt,3] fp32, held in double).  The source moves by init ([N,4,4] double, NULL = identity), then by
  *   each update; transformation = update * transformation.  A source point's correspondence is its nearest target point
