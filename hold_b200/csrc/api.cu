@@ -22,6 +22,7 @@
 #include "warp_bwd.cuh"
 #include "train.cuh"
 #include "wgrad_tc.cuh"
+#include "decimate.cuh"
 
 namespace hold {
 
@@ -391,6 +392,7 @@ int hold_ctx_check(hold_ctx* ctx, void* stream) {
   if (h & kErrNonFinite) { set_error("non-finite value (singular transform)"); return HOLD_E_NONFINITE; }
   if (h & kErrBadFace) { set_error("a face's vertex index is outside [0, V): the rasteriser skipped the face"); return HOLD_E_BADARG; }
   if (h & kErrBadLength) { set_error("a point-cloud length is outside [0, P]: the kernel clamped it"); return HOLD_E_BADARG; }
+  if (h & kErrBadMeshIndex) { set_error("a face's vertex index is outside [0, V): hold_decimate returned the mesh unchanged"); return HOLD_E_BADARG; }
   return HOLD_OK;
 }
 
@@ -1066,6 +1068,114 @@ int hold_icp(hold_ctx* ctx, int N, int Ps, const float* source, const int32_t* s
   }
   k_icp_out<<<pair_blocks, 128, 0, s>>>(a, transformation, fitness, inlier_rmse, iterations);
   HOLD_LAUNCH_CHECK(ctx);
+  return HOLD_OK;
+}
+
+int hold_decimate(hold_ctx* ctx, int V, const float* verts, int F, const int32_t* faces, int target_faces, float quality_threshold,
+                  float* verts_out, int32_t* faces_out, int* V_out_host, int* F_out_host, void* stream) {
+  HOLD_REQUIRE(ctx != nullptr, "ctx is NULL");
+  HOLD_REQUIRE(V >= 0 && F >= 0 && target_faces >= 0, "bad sizes V %d F %d target_faces %d", V, F, target_faces);
+  HOLD_REQUIRE((int64_t)F * 3 < (1ll << 31), "3 F = %lld half-edges is not below 2^31", (long long)F * 3);
+  HOLD_REQUIRE(!isnan(quality_threshold), "quality_threshold is NaN");
+  HOLD_REQUIRE(V_out_host && F_out_host && (V == 0 || (verts && verts_out)) && (F == 0 || (faces && faces_out)), "NULL argument");
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  const int n3 = 3 * F;
+  // one workspace, sized from the arguments
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_st = take(sizeof(DecState)), o_hist = take(256 * sizeof(int)), o_P = take((size_t)V * 3 * sizeof(float));
+  const size_t o_Q = take((size_t)V * 10 * sizeof(double)), o_F = take((size_t)n3 * sizeof(int)), o_fz = take((size_t)V * sizeof(int));
+  const size_t o_key = take((size_t)n3 * sizeof(uint64_t)), o_sel = take((size_t)n3 * sizeof(uint64_t));
+  const size_t o_mA = take((size_t)V * sizeof(uint64_t)), o_mB = take((size_t)V * sizeof(uint64_t));
+  const size_t o_X = take((size_t)n3 * 3 * sizeof(float)), o_sk = take((size_t)n3 * sizeof(int));
+  const size_t o_vn = take((size_t)(V + 1) * sizeof(int)), o_fn = take((size_t)(F + 1) * sizeof(int));
+  const size_t o_im = take(inverse_map_ints(n3, V) * sizeof(int));
+  WS(WS_DECIMATE, uint8_t, off, ws);
+  DecState* st = (DecState*)(ws + o_st);
+  int* hist = (int*)(ws + o_hist);
+  float* P = (float*)(ws + o_P);
+  double* Q = (double*)(ws + o_Q);
+  int *Fw = (int*)(ws + o_F), *frozen = (int*)(ws + o_fz), *skeys = (int*)(ws + o_sk), *vnew = (int*)(ws + o_vn), *fnew = (int*)(ws + o_fn);
+  uint64_t *key = (uint64_t*)(ws + o_key), *sel = (uint64_t*)(ws + o_sel), *mA = (uint64_t*)(ws + o_mA), *mB = (uint64_t*)(ws + o_mB);
+  float* X = (float*)(ws + o_X);
+  const int gF3 = ceil_div(max(n3, 1), kDecThreads), gV = ceil_div(max(V, 1), kDecThreads);
+  const int gSel = min(gF3, 4 * ctx->sm_count);
+  DecState h{};
+  auto read_state = [&]() -> int {
+    HOLD_CUDA(cudaMemcpyAsync(&h, st, sizeof(DecState), cudaMemcpyDeviceToHost, s));
+    HOLD_CUDA(cudaStreamSynchronize(s));
+    return HOLD_OK;
+  };
+  k_dec_state<<<1, 1, 0, s>>>(st, F, target_faces);
+  HOLD_LAUNCH_CHECK(ctx);
+  if (F > 0) {
+    k_dec_init<<<gF3, kDecThreads, 0, s>>>(n3, V, faces, Fw, st, ctx->dev_err);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  int rc = read_state();
+  if (rc) return rc;
+  if (h.bad || target_faces >= F) {
+    if (V) HOLD_CUDA(cudaMemcpyAsync(verts_out, verts, (size_t)V * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    if (F) HOLD_CUDA(cudaMemcpyAsync(faces_out, faces, (size_t)n3 * sizeof(int), cudaMemcpyDeviceToDevice, s));
+    *V_out_host = V, *F_out_host = F;
+    return HOLD_OK;
+  }
+  HOLD_CUDA(cudaMemcpyAsync(P, verts, (size_t)V * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  HOLD_CUDA(cudaMemsetAsync(hist, 0, 256 * sizeof(int), s));
+  auto select = [&](const uint64_t* keys, int which) -> int {
+    for (int pass = 0; pass < 8; ++pass) {
+      k_dec_sel_hist<<<gSel, kDecThreads, 0, s>>>(n3, keys, st, which, pass, hist);
+      HOLD_LAUNCH_CHECK(ctx);
+      k_dec_sel_pick<<<1, 1, 0, s>>>(st, which, pass, hist);
+      HOLD_LAUNCH_CHECK(ctx);
+    }
+    return HOLD_OK;
+  };
+  InvMap m;
+  for (int round = 0; round < kDecMaxRounds && h.F_live > target_faces; ++round) {
+    k_dec_star_keys<<<gF3, kDecThreads, 0, s>>>(n3, V, Fw, skeys);
+    HOLD_LAUNCH_CHECK(ctx);
+    if ((rc = inverse_map(ctx, skeys, n3, V, (int*)(ws + o_im), &m, s))) return rc;
+    if (round == 0) {
+      k_dec_quadrics<<<gV, kDecThreads, 0, s>>>(V, Fw, P, m, Q);
+      HOLD_LAUNCH_CHECK(ctx);
+    }
+    k_dec_frozen<<<gV, kDecThreads, 0, s>>>(V, Fw, m, frozen);
+    HOLD_LAUNCH_CHECK(ctx);
+    k_dec_edges<<<gF3, kDecThreads, 0, s>>>(n3, Fw, P, Q, m, frozen, (double)quality_threshold, key, X);
+    HOLD_LAUNCH_CHECK(ctx);
+    if ((rc = select(key, 0))) return rc;
+    k_dec_vmin<<<gV, kDecThreads, 0, s>>>(V, Fw, m, key, st, mA);
+    HOLD_LAUNCH_CHECK(ctx);
+    k_dec_ring<<<gV, kDecThreads, 0, s>>>(V, Fw, m, mA, mB);
+    HOLD_LAUNCH_CHECK(ctx);
+    k_dec_ring<<<gV, kDecThreads, 0, s>>>(V, Fw, m, mB, mA);
+    HOLD_LAUNCH_CHECK(ctx);
+    k_dec_select<<<gF3, kDecThreads, 0, s>>>(n3, Fw, key, st, mA, sel);
+    HOLD_LAUNCH_CHECK(ctx);
+    if ((rc = select(sel, 1))) return rc;
+    k_dec_apply<<<gF3, kDecThreads, 0, s>>>(n3, sel, st, Fw, P, Q, m, X);
+    HOLD_LAUNCH_CHECK(ctx);
+    if ((rc = read_state())) return rc;
+    if (h.collapses == 0) break;
+  }
+  // compaction: surviving vertices and faces in ascending input order
+  HOLD_CUDA(cudaMemsetAsync(vnew, 0, (size_t)(V + 1) * sizeof(int), s));
+  HOLD_CUDA(cudaMemsetAsync(fnew + F, 0, sizeof(int), s));
+  k_dec_flags<<<gF3, kDecThreads, 0, s>>>(F, Fw, vnew, fnew);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_im_scan<<<1, 1024, 0, s>>>(vnew, V + 1);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_im_scan<<<1, 1024, 0, s>>>(fnew, F + 1);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_dec_out_verts<<<gV, kDecThreads, 0, s>>>(V, vnew, P, verts_out);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_dec_out_faces<<<gF3, kDecThreads, 0, s>>>(F, fnew, vnew, Fw, faces_out);
+  HOLD_LAUNCH_CHECK(ctx);
+  HOLD_CUDA(cudaMemcpyAsync(V_out_host, vnew + V, sizeof(int), cudaMemcpyDeviceToHost, s));
+  HOLD_CUDA(cudaMemcpyAsync(F_out_host, fnew + F, sizeof(int), cudaMemcpyDeviceToHost, s));
+  HOLD_CUDA(cudaStreamSynchronize(s));
   return HOLD_OK;
 }
 

@@ -165,3 +165,23 @@ def generate_mesh(ctx, func, verts, level_set=0.0, res_init=32, res_up=3, keep_l
     if not keep_largest:
         return verts_mc, faces, normals, values
     return largest_component(verts_mc, faces)
+
+
+def decimate(ctx, verts, faces, target_faces: int, quality_threshold: float = 0.3):
+    """The object mesh brought down to `target_faces` faces by quadric edge collapse (hold_decimate), where the reference's
+    load_data calls pymeshlab's meshing_decimation_quadric_edge_collapse.  verts [V,3], faces [F,3] as numpy (generate_mesh's
+    output) or torch -> (verts [V',3] float32, faces [F',3] int32) on the context's device.  The result has target_faces or
+    target_faces - 1 faces unless the collapse rules stop it earlier; target_faces >= F returns the input unchanged.  Not
+    meshlab's result (DESIGN.md §6): the same rules in parallel rounds, bitwise reproducible.  A face index outside [0, V)
+    raises HoldError."""
+    dev = torch.device("cuda", ctx.device)
+    v = torch.as_tensor(verts).to(device=dev, dtype=torch.float32).reshape(-1, 3).contiguous()
+    f = torch.as_tensor(faces).to(device=dev, dtype=torch.int32).reshape(-1, 3).contiguous()
+    if int(target_faces) >= f.shape[0]:
+        return v, f
+    v_out, f_out = torch.empty_like(v), torch.empty_like(f)
+    nv, nf = C.c_int(0), C.c_int(0)
+    check(lib().hold_decimate(ctx.h, v.shape[0], ptr(v), f.shape[0], ptr(f), int(target_faces), C.c_float(quality_threshold),
+                              ptr(v_out), ptr(f_out), C.byref(nv), C.byref(nf), stream_ptr()))
+    ctx.check()
+    return v_out[: nv.value], f_out[: nf.value]

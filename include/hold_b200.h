@@ -241,6 +241,23 @@ int hold_icp(hold_ctx* ctx, int N, int Ps, const float* source, const int32_t* s
              const int32_t* tgt_lengths, const double* init, const hold_icp_cfg* cfg, double* transformation, double* fitness,
              double* inlier_rmse, int32_t* iterations, void* stream);
 
+/* Quadric edge-collapse decimation (Garland-Heckbert quadric error metrics; the rules are in hold_b200/csrc/decimate_phases.h):
+ * the object mesh of the pose refinement brought down to about target_faces faces, where the reference's load_data calls
+ * pymeshlab's meshing_decimation_quadric_edge_collapse.  Not meshlab's result: meshlab collapses in sequential greedy order,
+ * this collapses an independent set of the cheapest edges per round (hold_b200/csrc/decimate.cuh).
+ *   verts [V,3] fp32, faces [F,3] int32 (device) -> verts_out (capacity V), faces_out (capacity F), *V_out_host, *F_out_host.
+ *   Vertices on a boundary or non-manifold edge, or with a star of more than 24 faces, never move; a collapse keeps the link
+ *   condition, valences >= 3, face orientations and min(quality_threshold, the old star's worst) triangle quality
+ *   (4 sqrt(3) A / sum of squared edge lengths; meshlab's qualitythr default is 0.3).  Every collapse removes two faces: a
+ *   reachable target ends at target_faces or target_faces - 1 faces; the call stops earlier when no edge can collapse.  Output
+ *   order: the surviving vertices (those a surviving face uses) and faces, each in ascending input order.
+ *   target_faces >= F returns the input unchanged.  A face index outside [0, V) also returns it unchanged and sets the device
+ *   error word that hold_ctx_check reports as HOLD_E_BADARG.  3 F < 2^31, target_faces >= 0, else HOLD_E_BADARG.
+ *   Bitwise reproducible.  The workspace belongs to the context and only grows.  The call reads a count on the host once per
+ *   round (it synchronises the stream) and cannot be captured in a CUDA graph. */
+int hold_decimate(hold_ctx* ctx, int V, const float* verts, int F, const int32_t* faces, int target_faces, float quality_threshold,
+                  float* verts_out, int32_t* faces_out, int* V_out_host, int* F_out_host, void* stream);
+
 /* GPU Multiresolution IsoSurface Extraction (SURVEY §8f rank 4) — the class `mise.MISE` of code/src/libmise/mise.pyx (the
  * reference's only native code) as driven by generate_mesh (utils/meshing.py:9-72): same query / update / to_dense rounds,
  * same dense (R+1)^3 value grid, R = resolution_0 << depth, bit for bit; marching cubes stays with the caller (skimage).
