@@ -101,6 +101,7 @@ EXPORTS = {
     "hold_mc_emit": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, fp, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, fp, C.c_void_p, C.c_void_p]),
     "hold_mise_destroy": (C.c_int, [C.c_void_p]),
     "hold_mesh_sdf": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_int, fp, C.c_int, C.c_int, C.c_void_p, fp, C.c_void_p, C.c_void_p]),
+    "hold_mesh_sdf_bvh": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_int, fp, C.c_int, C.c_int, C.c_void_p, fp, C.c_void_p, C.c_void_p]),
     "hold_off_in_surface": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "hold_raster_silhouette": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, C.c_int, fp, C.c_int, C.c_int, C.POINTER(RasterCfg),
                                          fp, fp, fp, fp, C.c_void_p]),

@@ -15,6 +15,7 @@
 #include "background_tc.cuh"
 #include "pose_bwd.cuh"
 #include "mesh_sdf.cuh"
+#include "mesh_bvh.cuh"
 #include "raster.cuh"
 #include "pointcloud.cuh"
 #include "mise.cuh"
@@ -393,6 +394,7 @@ int hold_ctx_check(hold_ctx* ctx, void* stream) {
   if (h & kErrBadFace) { set_error("a face's vertex index is outside [0, V): the rasteriser skipped the face"); return HOLD_E_BADARG; }
   if (h & kErrBadLength) { set_error("a point-cloud length is outside [0, P]: the kernel clamped it"); return HOLD_E_BADARG; }
   if (h & kErrBadMeshIndex) { set_error("a face's vertex index is outside [0, V): hold_decimate returned the mesh unchanged"); return HOLD_E_BADARG; }
+  if (h & kErrBadSdfFace) { set_error("a face's vertex index is outside [0, V): hold_mesh_sdf_bvh wrote NaN and face -1"); return HOLD_E_BADARG; }
   return HOLD_OK;
 }
 
@@ -883,6 +885,61 @@ int hold_mesh_sdf(hold_ctx* ctx, int B, int P, const float* points, int V, const
   HOLD_REQUIRE(points && verts && faces && sdf, "NULL argument");
   dim3 grid(ceil_div(P, 128), B);
   k_mesh_sdf<<<grid, 128, 0, (cudaStream_t)stream>>>(P, V, F, verts_batched ? V * 3 : 0, points, verts, faces, sdf, face_idx);
+  HOLD_LAUNCH_CHECK(ctx);
+  return HOLD_OK;
+}
+
+int hold_mesh_sdf_bvh(hold_ctx* ctx, int B, int P, const float* points, int V, const float* verts, int verts_batched, int F,
+                      const int32_t* faces, float* sdf, int32_t* face_idx, void* stream) {
+  HOLD_REQUIRE(ctx != nullptr, "ctx is NULL");
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  HOLD_REQUIRE(B >= 0 && P >= 0 && V > 0 && F > 0, "bad sizes");
+  HOLD_REQUIRE(F <= meshbvh::kMaxFaces, "F = %d faces is over 2^24", F);
+  HOLD_REQUIRE(B <= 65535 && (int64_t)B * P < (1ll << 31), "bad sizes B %d P %d", B, P);
+  if (B == 0 || P == 0) return HOLD_OK;
+  HOLD_REQUIRE(points && verts && faces && sdf, "NULL argument");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int trees = verts_batched ? B : 1;
+  // one workspace, sized from the arguments
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_st = take(2 * sizeof(int)), o_bd = take((size_t)trees * 8 * sizeof(float));
+  const size_t o_codes = take((size_t)trees * F * sizeof(int)), o_order = take((size_t)trees * F * sizeof(int));
+  const size_t o_nodes = take((size_t)trees * 2 * F * 4 * sizeof(float4)), o_child = take((size_t)trees * F * sizeof(int2));
+  const size_t o_par = take((size_t)trees * 2 * F * sizeof(int)), o_vis = take((size_t)trees * F * sizeof(int));
+  const size_t o_sort = take(3 * (size_t)F * sizeof(int)), o_hist = take(radix_sort_hist_ints(F) * sizeof(int));
+  const size_t o_band = take((size_t)B * P * sizeof(int));
+  WS(WS_MESH_BVH, uint8_t, off, ws);
+  BvhArgs a{};
+  a.B = B, a.P = P, a.V = V, a.F = F, a.vstride = verts_batched ? V * 3 : 0, a.tstride = verts_batched ? 1 : 0;
+  a.points = points, a.verts = verts, a.faces = faces, a.sdf = sdf, a.face_idx = face_idx;
+  a.state = (int*)(ws + o_st), a.bounds = (float*)(ws + o_bd), a.codes = (int*)(ws + o_codes), a.order = (int*)(ws + o_order);
+  a.nodes = (float4*)(ws + o_nodes), a.child = (int2*)(ws + o_child), a.parent = (int*)(ws + o_par), a.visits = (int*)(ws + o_vis);
+  a.band = (int*)(ws + o_band), a.err = ctx->dev_err;
+  HOLD_CUDA(cudaMemsetAsync(a.state, 0, 2 * sizeof(int), s));
+  HOLD_CUDA(cudaMemsetAsync(a.visits, 0, (size_t)trees * F * sizeof(int), s));
+  k_bvh_bounds<<<trees, 1024, 0, s>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_bvh_codes<<<dim3(ceil_div(F, 256), trees), 256, 0, s>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  int* sb = (int*)(ws + o_sort);
+  for (int t = 0; t < trees; ++t) {
+    // 30 code bits: four passes, so the sorted faces land in vb[1], the tree's own order
+    int* const kb[2] = {sb, sb + F};
+    int* const vb[2] = {sb + 2 * (size_t)F, a.order + (size_t)t * F};
+    const int *kout, *vout;
+    int rc = radix_sort(ctx, a.codes + (size_t)t * F, F, 30, kb, vb, (int*)(ws + o_hist), &kout, &vout, s);
+    if (rc) return rc;
+    BvhArgs lt = a;
+    lt.sorted_codes = kout, lt.child = a.child + (size_t)t * F, lt.parent = a.parent + (size_t)t * 2 * F;
+    k_bvh_link<<<ceil_div(max(F - 1, 1), 256), 256, 0, s>>>(lt);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  k_bvh_refit<<<dim3(ceil_div(F, 256), trees), 256, 0, s>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_bvh_query<<<dim3(ceil_div(P, kBvhThreads), B), kBvhThreads, 0, s>>>(a);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_bvh_band<<<ceil_div(B * P, kBvhThreads), kBvhThreads, 0, s>>>(a);
   HOLD_LAUNCH_CHECK(ctx);
   return HOLD_OK;
 }

@@ -5,7 +5,8 @@
 // an item among the earlier items of its digit comes from __match_any_sync and per-warp counts in a fixed order, and the
 // tiles' bases from an exclusive scan of the (digit, tile) counts.  So the items of a key come out in ascending item order,
 // every position is a function of the keys alone, and no kernel uses an atomic.  The work is linear in the item count
-// whatever the keys: a key chosen by every item costs what distinct keys cost.
+// whatever the keys: a key chosen by every item costs what distinct keys cost.  The passes alone (radix_sort) also sort the
+// BVH's Morton codes (mesh_bvh.cuh).
 #pragma once
 #include "common.cuh"
 
@@ -122,15 +123,14 @@ inline size_t inverse_map_ints(int n, int nkeys) {
   return 4 * (size_t)n + (size_t)kImBins * ceil_div(max(n, 1), kImTile) + (size_t)nkeys + 1;
 }
 
-// keys [n] in [0, nkeys] -> *out, all of it inside ws (inverse_map_ints(n, nkeys) ints).  Launches only; sized from n and nkeys.
-inline int inverse_map(hold_ctx* ctx, const int* keys, int n, int nkeys, int* ws, InvMap* out, cudaStream_t s) {
+// ints of histogram radix_sort needs for n items
+inline size_t radix_sort_hist_ints(int n) { return (size_t)kImBins * ceil_div(max(n, 1), kImTile); }
+
+// Stable sort of the items [0, n) by the low `bits` bits of keys, ceil(bits / 8) passes ping-ponging through kb[] and vb[]
+// (n ints each; pass p writes kb[p & 1], vb[p & 1]).  On return *kout, *vout = the sorted keys and the item indices.
+inline int radix_sort(hold_ctx* ctx, const int* keys, int n, int bits, int* const kb[2], int* const vb[2], int* hist,
+                      const int** kout, const int** vout, cudaStream_t s) {
   const int tiles = ceil_div(max(n, 1), kImTile);
-  int* kb[2] = {ws, ws + n};
-  int* vb[2] = {ws + 2 * (size_t)n, ws + 3 * (size_t)n};
-  int* hist = ws + 4 * (size_t)n;
-  int* first = hist + (size_t)kImBins * tiles;
-  int bits = 1;
-  while (bits < 31 && (nkeys >> bits) != 0) ++bits;
   const int passes = ceil_div(bits, 8);
   const int* kin = keys;
   const int* vin = nullptr;
@@ -147,6 +147,21 @@ inline int inverse_map(hold_ctx* ctx, const int* keys, int n, int nkeys, int* ws
     }
     kin = ko, vin = vo;
   }
+  *kout = kin, *vout = vin;
+  return HOLD_OK;
+}
+
+// keys [n] in [0, nkeys] -> *out, all of it inside ws (inverse_map_ints(n, nkeys) ints).  Launches only; sized from n and nkeys.
+inline int inverse_map(hold_ctx* ctx, const int* keys, int n, int nkeys, int* ws, InvMap* out, cudaStream_t s) {
+  int* const kb[2] = {ws, ws + n};
+  int* const vb[2] = {ws + 2 * (size_t)n, ws + 3 * (size_t)n};
+  int* hist = ws + 4 * (size_t)n;
+  int* first = hist + radix_sort_hist_ints(n);
+  int bits = 1;
+  while (bits < 31 && (nkeys >> bits) != 0) ++bits;
+  const int *kin, *vin;
+  int rc = radix_sort(ctx, keys, n, bits, kb, vb, hist, &kin, &vin, s);
+  if (rc) return rc;
   k_im_first<<<ceil_div(nkeys + 1, 256), 256, 0, s>>>(kin, n, nkeys, first);
   HOLD_LAUNCH_CHECK(ctx);
   out->order = vin, out->first = first;

@@ -96,7 +96,7 @@ def compute_mano_cano_sdf(ctx, mesh_v_cano, mesh_f_cano, x_cano):
         v = v[0].contiguous()
     f = mesh_f_cano.to(torch.int32).contiguous()
     out = torch.empty(B, P, device=x.device)
-    check(lib().hold_mesh_sdf(ctx.h, B, P, ptr(x), v.shape[-2], ptr(v), int(batched), f.shape[0], ptr(f), ptr(out), None, stream_ptr()))
+    check(lib().hold_mesh_sdf_bvh(ctx.h, B, P, ptr(x), v.shape[-2], ptr(v), int(batched), f.shape[0], ptr(f), ptr(out), None, stream_ptr()))
     return out
 
 

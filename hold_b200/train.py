@@ -598,11 +598,12 @@ def prepare_loss_targets(out, node, B, P, canonical_pts, generator=None):
         if getattr(node, "mesh_v_cano_div", None) is None:
             return
         v = node.mesh_v_cano_div[None].repeat(B, 1, 1).float().contiguous()
+        v1 = node.mesh_v_cano_div.float().contiguous()                  # the SDF queries share one mesh: one tree, not B
         f = node.mesh_f_cano_div
         samples = pt_in_space_sampler_h.get_points(sample_on_barycentric_mesh(v, f, 256, generator), local_sigma=0.008, global_ratio=0.20, generator=generator)
         with torch.no_grad():
-            out[f"{nid}.pts2mano_sdf_cano"] = ops.compute_mano_cano_sdf(ctx, v, f, samples.contiguous())
-            off, _ = ops.check_off_in_surface_points_cano_mesh(ctx, v, f, canonical_pts.detach().reshape(B, -1, 3).contiguous(), B * P, threshold=0.01)
+            out[f"{nid}.pts2mano_sdf_cano"] = ops.compute_mano_cano_sdf(ctx, v1, f, samples.contiguous())
+            off, _ = ops.check_off_in_surface_points_cano_mesh(ctx, v1, f, canonical_pts.detach().reshape(B, -1, 3).contiguous(), B * P, threshold=0.01)
         sdf, _, _ = SdfNetFn.apply(node, samples.reshape(-1, 3).contiguous(), *Ws, *bs)            # query_oc (hold_utils.py:61-65)
         out[f"{nid}.pred_sdf"] = sdf.reshape(B, -1)
         out[f"{nid}.index_off_surface"] = off
@@ -613,7 +614,7 @@ def prepare_loss_targets(out, node, B, P, canonical_pts, generator=None):
             return
         v = node.mesh_vo_cano.reshape(1, -1, 3).repeat(B, 1, 1).float().contiguous()
         with torch.no_grad():
-            off, _ = ops.check_off_in_surface_points_cano_mesh(ctx, v, node.mesh_fo_cano, canonical_pts.detach().reshape(B, -1, 3).contiguous(), B * P, threshold=0.05)
+            off, _ = ops.check_off_in_surface_points_cano_mesh(ctx, v[0], node.mesh_fo_cano, canonical_pts.detach().reshape(B, -1, 3).contiguous(), B * P, threshold=0.05)
         out[f"{nid}.index_off_surface"] = off
         xyz = v[0].abs().max(0).values * 1.1
         out[f"{nid}.grad_theta"] = compute_gradient_samples(PointInSpace(global_sigma_xyz=xyz.cpu()), node, 256, v, B, 0.03, 0.20, generator)

@@ -170,6 +170,16 @@ int hold_object_tf_bwd(hold_ctx* ctx, int B, const float* rot, const float* tran
  * (verts [B,V,3] if verts_batched else [V,3] shared by all frames; faces [F,3] int32).  face_idx (nullable) = nearest face. */
 int hold_mesh_sdf(hold_ctx* ctx, int B, int P, const float* points, int V, const float* verts, int verts_batched, int F,
                   const int32_t* faces, float* sdf, int32_t* face_idx, void* stream);
+/* hold_mesh_sdf's arguments and results through a bounding-volume hierarchy (hold_b200/csrc/mesh_bvh.cuh): sdf and face_idx are
+ * bit for bit hold_mesh_sdf's, in O(log F) work per point instead of O(F).  Each call builds the tree (B trees when verts_batched)
+ * on the device, with no host synchronisation.  Points whose fast winding number lies within 0.25 of 0.5, and non-finite points,
+ * sum the exact solid angles over all faces as hold_mesh_sdf does.  F <= 2^24 and B P < 2^31, else HOLD_E_BADARG.  A face index
+ * outside [0, V) gives NaN sdf and face -1 for every point and sets the device error word that hold_ctx_check reports as
+ * HOLD_E_BADARG.  The tree lives in a context workspace that only grows, so after one eager call at the same or larger sizes
+ * (B, P, F and verts_batched) the call can be captured in a CUDA graph.  All calls on one context share the workspace: issue them
+ * on one stream (or order them across streams). */
+int hold_mesh_sdf_bvh(hold_ctx* ctx, int B, int P, const float* points, int V, const float* verts, int verts_batched, int F,
+                      const int32_t* faces, float* sdf, int32_t* face_idx, void* stream);
 /* The per-ray reduction of check_off_in_surface_points_cano_mesh (volsdf_utils.py:209-217): over the S samples of each of
  * R rays, off_surface = min sdf > threshold, in_surface = min sdf <= 0 (uint8 flags, each output nullable). */
 int hold_off_in_surface(hold_ctx* ctx, int R, int S, const float* sdf, float threshold, uint8_t* off_surface,
