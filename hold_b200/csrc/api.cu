@@ -1251,7 +1251,7 @@ int hold_inverse_warp_bwd(hold_ctx* ctx, int node, int B, int P, const float* x,
   if ((rc = ws_get(ctx, WS_WARPBWD,(size_t)B * nb * warpbwd::kJ * warpbwd::kG * sizeof(float), &part))) return rc;
   dim3 grid(nb, B);
   if (hand) {
-    HOLD_REQUIRE(ns.has_rig, "hand node has no rig (hold_node_set_rig)");
+    if (!ns.has_rig) { set_error("hand node has no rig (hold_node_set_rig)"); return HOLD_E_STATE; }
     HOLD_REQUIRE(P == 0 || (knn_idx && pose->posed_verts), "hand backward needs the forward's knn_idx and the posed vertices");
     k_inverse_warp_bwd_hand<<<grid, 128, 0, s>>>(P, x, knn_idx, pose->posed_verts, ns.skin_w, pose->tfs, g_xc, g_x, (float*)part);
     HOLD_LAUNCH_CHECK(ctx);
