@@ -112,6 +112,7 @@ EXPORTS = {
     "hold_icp": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, C.c_int, fp, fp, fp, C.POINTER(IcpCfg), fp, fp, fp, fp, C.c_void_p]),
     "hold_decimate": (C.c_int, [C.c_void_p, C.c_int, fp, C.c_int, fp, C.c_int, C.c_float, fp, fp, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                 C.c_void_p]),
+    "hold_largest_component": (C.c_int, [C.c_void_p, C.c_int, fp, C.c_int, fp, fp, fp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
     "hold_mano_lbs_bwd": (C.c_int, [C.c_void_p, C.POINTER(ManoModel), C.c_int] + [fp] * 12 + [C.c_void_p]),
     "hold_object_tf_bwd": (C.c_int, [C.c_void_p, C.c_int, fp, fp, fp, C.c_float, fp, fp, C.c_int] + [fp] * 6 + [C.c_void_p]),
     "hold_camera_rays": (C.c_int, [C.c_void_p, C.c_int, C.c_int, fp, fp, fp, fp, fp, C.c_void_p]),

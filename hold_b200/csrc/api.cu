@@ -24,6 +24,7 @@
 #include "train.cuh"
 #include "wgrad_tc.cuh"
 #include "decimate.cuh"
+#include "mesh_cc.cuh"
 
 namespace hold {
 
@@ -395,6 +396,7 @@ int hold_ctx_check(hold_ctx* ctx, void* stream) {
   if (h & kErrBadLength) { set_error("a point-cloud length is outside [0, P]: the kernel clamped it"); return HOLD_E_BADARG; }
   if (h & kErrBadMeshIndex) { set_error("a face's vertex index is outside [0, V): hold_decimate returned the mesh unchanged"); return HOLD_E_BADARG; }
   if (h & kErrBadSdfFace) { set_error("a face's vertex index is outside [0, V): hold_mesh_sdf_bvh wrote NaN and face -1"); return HOLD_E_BADARG; }
+  if (h & kErrBadCcFace) { set_error("a face's vertex index is outside [0, V): hold_largest_component returned an empty mesh"); return HOLD_E_BADARG; }
   return HOLD_OK;
 }
 
@@ -1233,6 +1235,77 @@ int hold_decimate(hold_ctx* ctx, int V, const float* verts, int F, const int32_t
   HOLD_CUDA(cudaMemcpyAsync(V_out_host, vnew + V, sizeof(int), cudaMemcpyDeviceToHost, s));
   HOLD_CUDA(cudaMemcpyAsync(F_out_host, fnew + F, sizeof(int), cudaMemcpyDeviceToHost, s));
   HOLD_CUDA(cudaStreamSynchronize(s));
+  return HOLD_OK;
+}
+
+int hold_largest_component(hold_ctx* ctx, int V, const float* verts, int F, const int32_t* faces, float* verts_out,
+                           int32_t* faces_out, int* V_out_host, int* F_out_host, void* stream) {
+  HOLD_REQUIRE(ctx != nullptr, "ctx is NULL");
+  HOLD_REQUIRE(V >= 0 && F >= 0, "bad sizes V %d F %d", V, F);
+  HOLD_REQUIRE((int64_t)F * 3 < (1ll << 31), "3 F = %lld corners is not below 2^31", (long long)F * 3);
+  HOLD_REQUIRE(V_out_host && F_out_host && (V == 0 || (verts && verts_out)) && (F == 0 || (faces && faces_out)), "NULL argument");
+  HOLD_CUDA(cudaSetDevice(ctx->device));
+  *V_out_host = 0, *F_out_host = 0;
+  if (F == 0) return HOLD_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int n3 = 3 * F;
+  // one workspace, sized from the arguments
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_st = take(sizeof(CcState)), o_par = take((size_t)V * sizeof(int)), o_lab = take((size_t)V * sizeof(int));
+  const size_t o_area = take((size_t)F * sizeof(float));
+  const size_t o_key = take((size_t)F * sizeof(int)), o_sum = take((size_t)V * sizeof(double));
+  const size_t o_vn = take((size_t)(V + 1) * sizeof(int)), o_fn = take((size_t)(F + 1) * sizeof(int));
+  const size_t o_im = take(inverse_map_ints(F, V) * sizeof(int));
+  WS(WS_MESH_CC, uint8_t, off, ws);
+  CcState* st = (CcState*)(ws + o_st);
+  int *parent = (int*)(ws + o_par), *label = (int*)(ws + o_lab), *key = (int*)(ws + o_key), *vnew = (int*)(ws + o_vn), *fnew = (int*)(ws + o_fn);
+  float* area = (float*)(ws + o_area);
+  double* sums = (double*)(ws + o_sum);
+  const int gF = ceil_div(F, kCcThreads), gV = ceil_div(max(V, 1), kCcThreads);
+  HOLD_CUDA(cudaMemsetAsync(st, 0, sizeof(CcState), s));
+  k_cc_init<<<ceil_div(max(V, n3), kCcThreads), kCcThreads, 0, s>>>(V, n3, faces, parent, st, ctx->dev_err);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_cc_unite<<<gF, kCcThreads, 0, s>>>(F, faces, parent, st);
+  HOLD_LAUNCH_CHECK(ctx);
+  if (V > 0) {
+    k_cc_labels<<<gV, kCcThreads, 0, s>>>(V, parent, st, label);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  k_cc_area<<<gF, kCcThreads, 0, s>>>(F, V, verts, faces, label, st, area, key);
+  HOLD_LAUNCH_CHECK(ctx);
+  InvMap m;
+  int rc = inverse_map(ctx, key, F, V, (int*)(ws + o_im), &m, s);
+  if (rc) return rc;
+  if (V > 0) {
+    k_cc_sums<<<gV, kCcThreads, 0, s>>>(V, area, m, sums);
+    HOLD_LAUNCH_CHECK(ctx);
+    k_cc_argmax<<<1, kCcArgmaxThreads, 0, s>>>(V, sums, st);
+    HOLD_LAUNCH_CHECK(ctx);
+  } else {
+    HOLD_CUDA(cudaMemsetAsync(&st->best, 0xff, sizeof(int), s));   // every face is out of range: -1, nothing kept
+  }
+  // compaction: kept vertices in ascending old id, kept faces in input order
+  HOLD_CUDA(cudaMemsetAsync(vnew, 0, (size_t)(V + 1) * sizeof(int), s));
+  HOLD_CUDA(cudaMemsetAsync(fnew + F, 0, sizeof(int), s));
+  k_cc_flags<<<gF, kCcThreads, 0, s>>>(F, faces, label, st, vnew, fnew);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_im_scan<<<1, 1024, 0, s>>>(vnew, V + 1);
+  HOLD_LAUNCH_CHECK(ctx);
+  k_im_scan<<<1, 1024, 0, s>>>(fnew, F + 1);
+  HOLD_LAUNCH_CHECK(ctx);
+  if (V > 0) {
+    k_cc_out_verts<<<gV, kCcThreads, 0, s>>>(V, vnew, verts, verts_out);
+    HOLD_LAUNCH_CHECK(ctx);
+  }
+  k_cc_out_faces<<<gF, kCcThreads, 0, s>>>(F, fnew, vnew, faces, faces_out);
+  HOLD_LAUNCH_CHECK(ctx);
+  // the one host read: the two output sizes
+  int sizes[2];
+  HOLD_CUDA(cudaMemcpyAsync(&sizes[0], vnew + V, sizeof(int), cudaMemcpyDeviceToHost, s));
+  HOLD_CUDA(cudaMemcpyAsync(&sizes[1], fnew + F, sizeof(int), cudaMemcpyDeviceToHost, s));
+  HOLD_CUDA(cudaStreamSynchronize(s));
+  *V_out_host = sizes[0], *F_out_host = sizes[1];
   return HOLD_OK;
 }
 

@@ -28,6 +28,7 @@ constexpr int kErrBadFace = 4;   // a face's vertex index is outside [0, V) (the
 constexpr int kErrBadLength = 8; // a point-cloud length is outside [0, P] (the KNN / ICP kernels clamp it)
 constexpr int kErrBadMeshIndex = 16; // a face's vertex index is outside [0, V) (hold_decimate returns the mesh unchanged)
 constexpr int kErrBadSdfFace = 32;   // a face's vertex index is outside [0, V) (hold_mesh_sdf_bvh wrote NaN and -1)
+constexpr int kErrBadCcFace = 64;    // a face's vertex index is outside [0, V) (hold_largest_component returned an empty mesh)
 
 struct SamplerState {  // device-resident, one per node; written only by single-thread epilogues
   int iters;           // rounds executed so far
@@ -55,7 +56,7 @@ struct PackedNet {
 // grow-only workspaces of a hold_ctx, one per purpose
 enum WsSlot { WS_Z = 0, WS_SDF, WS_ZNEW, WS_SDFNEW, WS_BETA, WS_FAR, WS_XC, WS_SSDF, WS_GRAD, WS_FEAT, WS_PE, WS_ZTMP, WS_SIG,
               WS_BGSDF, WS_BGFEAT, WS_BGRGB, WS_AMAX, WS_WARPBWD, WS_RASTER, WS_ICP, WS_WGRAD,
-              WS_RASTER_BWD, WS_KNN_BWD, WS_DECIMATE, WS_MESH_BVH, WS_COUNT };
+              WS_RASTER_BWD, WS_KNN_BWD, WS_DECIMATE, WS_MESH_BVH, WS_MESH_CC, WS_COUNT };
 
 struct NodeState {
   bool configured = false, has_weights = false, has_rig = false;

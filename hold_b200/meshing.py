@@ -57,10 +57,9 @@ class MISE:
             pass
 
 
-def generate_grid(ctx, func, verts, level_set=0.0, res_init=32, res_up=3, scale=1.1):
-    """The value grid `generate_mesh` hands to marching cubes (utils/meshing.py:10-47).  `func(points [n,3] cuda float32)`
-    returns their SDF ([n] or {"sdf": ...}); `verts` = canonical mesh vertices (numpy / tensor [V,3]) for the bounding box.
-    Returns (value_grid float64 numpy [(R+1)^3 as R+1 cubed], resolution, gt_scale, gt_center)."""
+def _dense_grid(ctx, func, verts, level_set, res_init, res_up, scale):
+    """The MISE rounds of `generate_grid` -> (value grid float32 [(R+1)^3 as R+1 cubed] on the device, resolution, gt_scale,
+    gt_center)."""
     v = np.asarray(verts.detach().cpu() if torch.is_tensor(verts) else verts, dtype=np.float32)
     gt_bbox = np.stack([v.min(axis=0), v.max(axis=0)], axis=0)
     gt_center = (gt_bbox[0] + gt_bbox[1]) * 0.5
@@ -77,17 +76,27 @@ def generate_grid(ctx, func, verts, level_set=0.0, res_init=32, res_up=3, scale=
         pts = pts * float(gt_scale) + center
         out = func(pts.contiguous())
         ex.update(coords, out["sdf"] if isinstance(out, dict) else out)
-    grid = ex.to_dense().cpu().numpy().astype(np.float64)
+    grid = ex.to_dense()
     res = ex.resolution
+    torch.cuda.current_stream().synchronize()              # to_dense reads the octree that close() frees
     ex.close()
     return grid, res, gt_scale, gt_center
 
 
-def node_sdf_func(ctx, node):
-    """`lambda x: query_oc(implicit_network, x, cond)` of hold.py:139-167 for a hold_b200 Node: SDF of canonical points."""
+def generate_grid(ctx, func, verts, level_set=0.0, res_init=32, res_up=3, scale=1.1):
+    """The value grid `generate_mesh` hands to marching cubes (utils/meshing.py:10-47).  `func(points [n,3] cuda float32)`
+    returns their SDF ([n] or {"sdf": ...}); `verts` = canonical mesh vertices (numpy / tensor [V,3]) for the bounding box.
+    Returns (value_grid float64 numpy [(R+1)^3 as R+1 cubed], resolution, gt_scale, gt_center)."""
+    grid, res, gt_scale, gt_center = _dense_grid(ctx, func, verts, level_set, res_init, res_up, scale)
+    return grid.cpu().numpy().astype(np.float64), res, gt_scale, gt_center
+
+
+def node_sdf_func(ctx, node, embed_w=None):
+    """`lambda x: query_oc(implicit_network, x, cond)` of hold.py:139-167 for a hold_b200 Node: SDF of canonical points.
+    embed_w: the BARF weights [39] of the object's embedder (Node.embed_w()); None = every frequency passes."""
     def f(pts):
         sdf = torch.empty(pts.shape[0], device=pts.device)
-        check(lib().hold_sdf_eval(ctx.h, node.slot, pts.shape[0], ptr(pts), None, ptr(sdf), None, None, stream_ptr()))
+        check(lib().hold_sdf_eval(ctx.h, node.slot, pts.shape[0], ptr(pts), ptr(embed_w), ptr(sdf), None, None, stream_ptr()))
         return sdf
     return f
 
@@ -115,6 +124,23 @@ def largest_component(verts, faces):
     return verts[used], remap[f[keep_f]]
 
 
+def largest_component_device(ctx, verts, faces):
+    """`largest_component` on the device (hold_largest_component), bit for bit: verts [V,3], faces [F,3] (numpy or torch) ->
+    (verts [V',3] float32, faces [F',3] int32) on the context's device.  No face raises ValueError, as np.argmax of no component
+    does; a face index outside [0, V) raises HoldError."""
+    dev = torch.device("cuda", ctx.device)
+    v = torch.as_tensor(verts).to(device=dev, dtype=torch.float32).reshape(-1, 3).contiguous()
+    f = torch.as_tensor(faces).to(device=dev, dtype=torch.int32).reshape(-1, 3).contiguous()
+    if f.shape[0] == 0:
+        raise ValueError("attempt to get argmax of an empty sequence: the mesh has no face")
+    v_out, f_out = torch.empty_like(v), torch.empty_like(f)
+    nv, nf = C.c_int(0), C.c_int(0)
+    check(lib().hold_largest_component(ctx.h, v.shape[0], ptr(v), f.shape[0], ptr(f), ptr(v_out), ptr(f_out), C.byref(nv),
+                                       C.byref(nf), stream_ptr()))
+    ctx.check()
+    return v_out[: nv.value], f_out[: nf.value]
+
+
 def marching_cubes(ctx, volume: torch.Tensor, level: float = 0.0):
     """(verts [Nv,3] float32 in index coordinates, faces [Nt,3] int32) of the level set of a dense grid on the device (hold_mc_mark /
     hold_mc_emit + two torch.cumsum scans).  Inside = value < level; normals (right-hand rule) towards increasing values."""
@@ -137,24 +163,45 @@ def marching_cubes(ctx, volume: torch.Tensor, level: float = 0.0):
     return verts, faces
 
 
+def grid_to_world(verts, res, gt_scale, gt_center):
+    """Marching-cubes index coordinates [n,3] float32 (device) -> the bounding box of generate_grid (utils/meshing.py:52-53):
+    ((v / res - 0.5) * 1.1) * gt_scale + gt_center, in float32 one operation at a time, as numpy rounds it.  res is divided as
+    a device tensor: torch multiplies by the reciprocal of a host scalar divisor, which rounds differently."""
+    res_t = torch.full((), float(res), device=verts.device)
+    center = torch.from_numpy(np.asarray(gt_center, np.float32)).to(verts.device)
+    return ((verts / res_t - 0.5) * 1.1) * float(gt_scale) + center
+
+
+def extract_mesh(ctx, func, verts, level_set=0.0, res_init=32, res_up=3):
+    """generate_mesh(backend="gpu") kept on the device: the MISE grid (float32, the values generate_grid's float64 grid holds),
+    marching_cubes, grid_to_world and largest_component_device -> (verts [n,3] float32, faces [m,3] int32), device tensors.
+    An empty level set raises ValueError, as generate_mesh's np.argmax does."""
+    grid, res, gt_scale, gt_center = _dense_grid(ctx, func, verts, level_set, res_init, res_up, 1.1)
+    v, f = marching_cubes(ctx, grid, level_set)
+    return largest_component_device(ctx, grid_to_world(v, res, gt_scale, gt_center), f)
+
+
 def generate_mesh(ctx, func, verts, level_set=0.0, res_init=32, res_up=3, keep_largest=True, backend="auto"):
     """utils/meshing.py:9-72 -> (verts [n,3], faces [m,3]) of the largest connected component (keep_largest=False: the raw
     marching-cubes tuple (verts, faces, normals, values)).  backend: "skimage" (the reference's call), "gpu" (hold_mc_*), "auto" =
-    skimage when importable, else gpu.  The component selection (trimesh in the reference) is `largest_component` above."""
-    grid, res, gt_scale, gt_center = generate_grid(ctx, func, verts, level_set, res_init, res_up)
+    skimage when importable, else gpu.  The component selection (trimesh in the reference) is `largest_component` above, and on
+    the gpu backend its device equal `largest_component_device`: the gpu result is `extract_mesh`'s, copied to the host."""
     if backend == "auto":
         try:
             import skimage.measure  # noqa: F401  (the reference's own dependency for this step)
             backend = "skimage"
         except ImportError:
             backend = "gpu"
+    if backend == "gpu" and keep_largest:
+        v, f = extract_mesh(ctx, func, verts, level_set, res_init, res_up)
+        return v.cpu().numpy(), f.cpu().numpy().astype(np.int64)
+    grid, res, gt_scale, gt_center = generate_grid(ctx, func, verts, level_set, res_init, res_up)
     if backend == "gpu":
         # hold_mc_*: outward normals (towards increasing SDF); normals / values of the skimage tuple are not produced
         dev = torch.device("cuda", ctx.device)
         v, f = marching_cubes(ctx, torch.as_tensor(grid, device=dev), level_set)
         verts_mc = ((v.cpu().numpy() / res - 0.5) * 1.1) * gt_scale + gt_center
-        faces = f.cpu().numpy().astype(np.int64)
-        return largest_component(verts_mc, faces) if keep_largest else (verts_mc, faces, None, None)
+        return verts_mc, f.cpu().numpy().astype(np.int64), None, None
     from skimage import measure
 
     mc = getattr(measure, "marching_cubes_lewiner", None) or measure.marching_cubes

@@ -347,6 +347,21 @@ class Node(nn.Module):
         # back only to later work of that same stream (a sync here stalled every training step three times and made the step
         # uncapturable as a CUDA graph)
 
+    def meshing_cano(self, res_init=32, res_up=3):
+        """The node's canonical mesh from its current SDF, as HOLD.meshing_cano builds it (hold.py:139-167) -> (verts [n,3]
+        float32, faces [m,3] int32) on the device (meshing.extract_mesh).  The weights are re-packed first, as every training
+        step does, and the SDF is queried as ImplicitNet.forward does, with the current BARF mask of the object's embedder.
+        The bounding box is the server's canonical vertices.  The object node keeps the mesh as mesh_vo_cano / mesh_fo_cano,
+        the loss targets' mesh (train.prepare_loss_targets); a hand's targets use the MANO mesh, so a hand only returns it."""
+        from . import meshing
+
+        self.sync_weights()
+        f = meshing.node_sdf_func(self.ctx, self, embed_w=self.embed_w())
+        v, fc = meshing.extract_mesh(self.ctx, f, self.server.verts_c[0], res_init=res_init, res_up=res_up)
+        if self.kind == "object":
+            self.mesh_vo_cano, self.mesh_fo_cano = v, fc
+        return v, fc
+
     # -- articulation ---------------------------------------------------------------------------------
     def articulate(self, input):
         """The server call at the top of sample_points (mano_node.py:72-79 / object_node.py:58-62) -> NodePose."""

@@ -617,7 +617,19 @@ def prepare_loss_targets(out, node, B, P, canonical_pts, generator=None):
             off, _ = ops.check_off_in_surface_points_cano_mesh(ctx, v[0], node.mesh_fo_cano, canonical_pts.detach().reshape(B, -1, 3).contiguous(), B * P, threshold=0.05)
         out[f"{nid}.index_off_surface"] = off
         xyz = v[0].abs().max(0).values * 1.1
-        out[f"{nid}.grad_theta"] = compute_gradient_samples(PointInSpace(global_sigma_xyz=xyz.cpu()), node, 256, v, B, 0.03, 0.20, generator)
+        # the box stays on the device (the same values as a host copy), so a step with the object's mesh can be graph-captured
+        out[f"{nid}.grad_theta"] = compute_gradient_samples(PointInSpace(global_sigma_xyz=xyz), node, 256, v, B, 0.03, 0.20, generator)
+
+
+def meshing_cano(net, res_init=32, res_up=3):
+    """HOLD.meshing_cano (hold.py:139-167): every node's canonical mesh rebuilt from its current SDF (Node.meshing_cano), the
+    object's attached for the loss targets -> {node_id: (verts, faces)} on the device.  Writes no file.  A TrainStep captured
+    before the refresh must be captured again (TrainStep.replay raises)."""
+    return {nid: node.meshing_cano(res_init, res_up) for nid, node in net.nodes.items()}
+
+
+# the canonical-mesh attributes prepare_loss_targets reads
+MESH_ATTRS = ("mesh_v_cano_div", "mesh_f_cano_div", "mesh_vo_cano", "mesh_fo_cano")
 
 
 def forward_train(net, input, generator=None, stratified=False):
@@ -779,10 +791,21 @@ class TrainStep:
         self.opt.zero_grad(set_to_none=False)
         with torch.cuda.graph(self._graph):
             self._loss, self._parts = self.step(self._static, *self._gt, zero=True)
+        # the graph holds raw pointers to the canonical meshes it was captured with (their sizes are baked into it too)
+        self._meshes = {(nid, a): getattr(node, a, None) for nid, node in self.net.nodes.items() for a in MESH_ATTRS}
         return self
 
+    def _check_meshes(self):
+        for (nid, a), t in self._meshes.items():
+            if getattr(self.net.nodes[nid], a, None) is not t:
+                raise RuntimeError(f"node {nid!r}: {a} is not the tensor this step was captured with (a mesh refresh such as "
+                                   "train.meshing_cano replaces it, and the graph would read the old mesh's freed memory): "
+                                   "call capture() again")
+
     def replay(self, input=None, gt_rgb=None, gt_mask=None):
-        """One captured step; new batch contents (same shapes) are copied into the captured tensors first."""
+        """One captured step; new batch contents (same shapes) are copied into the captured tensors first.  Raises when a
+        node's canonical mesh is no longer the tensor the step was captured with."""
+        self._check_meshes()
         if input is not None:
             for k, v in input.items():
                 if torch.is_tensor(v) and k not in self._leaf_of:

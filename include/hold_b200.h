@@ -268,6 +268,19 @@ int hold_icp(hold_ctx* ctx, int N, int Ps, const float* source, const int32_t* s
 int hold_decimate(hold_ctx* ctx, int V, const float* verts, int F, const int32_t* faces, int target_faces, float quality_threshold,
                   float* verts_out, int32_t* faces_out, int* V_out_host, int* F_out_host, void* stream);
 
+/* The connected component of largest surface area, where the reference's generate_mesh calls trimesh.split and takes the argmax
+ * of the areas (utils/meshing.py:58-70).  Bit for bit hold_b200.meshing.largest_component (the rules are in
+ * hold_b200/csrc/mesh_cc_phases.h): components over the face edges, face areas in float32 as numpy rounds them, per-component
+ * sums in double in ascending face order, ties to the component with the smaller smallest vertex id.
+ *   verts [V,3] fp32, faces [F,3] int32 (device) -> verts_out (capacity V): the kept vertices in ascending input order;
+ *   faces_out (capacity F): the kept faces in input order, re-indexed; *V_out_host, *F_out_host.  When every area is 0 the
+ *   component of vertex 0 is kept, which has no face if vertex 0 is unused.  F == 0 gives two zero sizes.  A face index outside
+ *   [0, V) gives an empty result and sets the device error word that hold_ctx_check reports as HOLD_E_BADARG.  3 F < 2^31,
+ *   else HOLD_E_BADARG.  Bitwise reproducible: no floating-point atomic.  The workspace belongs to the context and only grows.
+ *   The call reads the two sizes on the host once at the end (it synchronises the stream). */
+int hold_largest_component(hold_ctx* ctx, int V, const float* verts, int F, const int32_t* faces, float* verts_out,
+                           int32_t* faces_out, int* V_out_host, int* F_out_host, void* stream);
+
 /* GPU Multiresolution IsoSurface Extraction (SURVEY §8f rank 4) — the class `mise.MISE` of code/src/libmise/mise.pyx (the
  * reference's only native code) as driven by generate_mesh (utils/meshing.py:9-72): same query / update / to_dense rounds,
  * same dense (R+1)^3 value grid, R = resolution_0 << depth, bit for bit; marching cubes stays with the caller (skimage).
